@@ -34,6 +34,9 @@ UNIT = "pairs/s"
 # algorithmic bytes per pair of the phase-1 kernel (DESIGN.md "roofline"):
 #   2 handles (8) + 2 poses (192) + 2 shape records (80) + 1 result record (96)
 BYTES_PER_PAIR = 8 + 192 + 80 + 96
+# --dump-outputs: rows kept of a larger result (float64 columns incl. the row number: config 2 writes 15 per row, 31 MB
+# at 256 Ki rows; config 5 22, 46 MB; both under 64 MB)
+DUMP_ROWS = 1 << 18
 
 
 def parse():
@@ -48,7 +51,14 @@ def parse():
                     help="0 DefaultGJK, 1 Polyak, 2 NesterovAcceleration (default: 0; config3: 2, as BASELINE names it)")
     ap.add_argument("--cpu-sample", type=int, default=400_000)
     ap.add_argument("--cpu-threads", type=int, default=0, help="threads of the CPU arm (0: calibrated)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result records of the last timed step to DIR/<field>.npy (float64, a fixed "
+                         "seeded sample of at most %d rows)" % DUMP_ROWS)
     a = ap.parse_args()
+    if a.dump_outputs and a.gpus != 1:
+        ap.error("--dump-outputs needs --gpus 1")
+    if a.dump_outputs and a.steps < 1:
+        ap.error("--dump-outputs needs --steps 1 or more (it writes what the last timed step computed)")
     if a.variant is None:
         a.variant = 2 if a.workload == "config3" else 0
     if a.workload == "config4" and a.pairs == 1_000_000:
@@ -65,7 +75,7 @@ def env_rank():
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -239,7 +249,7 @@ def run_reference(args):
 
 def support_kernel_roofline(eng_factory, peak, n_hulls=786432, nv=64, n_queries=1 << 21):
     """The north_star's convex-support kernel: batched ConvexBase support argmax over DISTINCT hulls
-    (1.2 GB of vertices, ten times the 126 MB L2, each hull queried 2.7 times on average, so the
+    (1.2 GB of vertices, 24 times the 50 MB L2 of an H100, each hull queried 2.7 times on average, so the
     algorithmic bytes are close to what DRAM delivers), one warp per query, coalesced SoA rows.
     Algorithmic bytes per query: 24*nv vertices + 24 B direction + 28 B output + 4 B id (SURVEY 8d:
     1 588 B at nv = 64)."""
@@ -288,22 +298,28 @@ def _peak():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    src = "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    src = "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet: 3.35 TB/s"
     return peak, src
 
 
-def _traffic(workload, n, variant):
-    """DRAM bytes of the dominant kernel per full-size launch, from the committed ncu capture of this command
-    (profiles/r02_dominant_kernel_traffic.json; a profiler run, not measured live)"""
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_dominant_kernel_traffic.json")))
-        e = tj[workload]
-        if n == e.get("pairs") and variant == e.get("variant", variant):
-            return e["traffic"], e.get("source")
-    except Exception:
-        pass
-    return None, None
+def dump_records(out_dir, recs, extra=None):
+    """recs: the result records one call of the timed path returned.  Every field (padding aside) becomes
+    out_dir/<field>.npy in float64; above DUMP_ROWS rows a fixed, seeded sample of rows is kept, and its row
+    numbers go to out_dir/row.npy.  `extra`: further arrays of the same rows (name -> array)."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(recs)
+    rows = np.arange(n)
+    if n > DUMP_ROWS:
+        rows = np.sort(np.random.default_rng(0x5EED).choice(n, DUMP_ROWS, replace=False))
+    cols = {"row": rows}
+    for f in recs.dtype.names:
+        if not f.startswith("_"):
+            cols[f] = recs[f][rows]
+    for k, v in (extra or {}).items():
+        cols[k] = np.asarray(v)[rows]
+    for k, v in cols.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.asarray(v, dtype=np.float64))
 
 
 def measure(args, workload, rank, local, world, dist, steps, warmup, clocks=False):
@@ -330,7 +346,7 @@ def measure(args, workload, rank, local, world, dist, steps, warmup, clocks=Fals
     out_bytes = n * P.distance_result_dtype.itemsize
     d_out = torch.empty(out_bytes, dtype=torch.uint8, device="cuda") if world == 1 else None
     stream = torch.cuda.current_stream().cuda_stream
-    # config 4's working set (34 MB) fits the 126 MB L2: flush it between steps by overwriting 256 MB
+    # config 4's working set (34 MB) fits the 50 MB L2: flush it between steps by overwriting 256 MB
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda") if workload == "config4" else None
     if world > 1:
         # the product's communicator: every step's records are all-gathered by the library (NCCL, on its own stream,
@@ -376,6 +392,8 @@ def measure(args, workload, rank, local, world, dist, steps, warmup, clocks=Fals
     barrier()
     ms = e0.elapsed_time(e1)
     st1 = eng.stats()
+    if args.dump_outputs and workload == args.workload:
+        dump_records(args.dump_outputs, d_out.cpu().numpy().view(P.distance_result_dtype))
     if world > 1:
         t = torch.tensor([ms], device="cuda", dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -499,9 +517,8 @@ def measure(args, workload, rank, local, world, dist, steps, warmup, clocks=Fals
         bpp = 2 * 1536 + 192 + 8 + 96
     k_ms = dom_ms / max(1, dom_launches)
     achieved = bpp * units / (k_ms * 1e-3) / 1e9 if k_ms > 0 else None
-    traffic, tsrc = _traffic(workload, n, variant)
     res["roofline"] = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                       "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": tsrc,
+                       "frac": (achieved / peak) if achieved else None,
                        "bytes_per_pair": bpp, "pairs_per_launch": units, "kernel_ms": k_ms, "peak_source": peak_src,
                        "timing": "CUDA events around the kernel's launches on the launching stream, in a separate pass "
                                  "of %d steps after the timed region" % prof_steps}
@@ -514,19 +531,19 @@ def measure(args, workload, rank, local, world, dist, steps, warmup, clocks=Fals
                       "epa_pairs_per_step": (sp1["epa_pairs"] - sp0["epa_pairs"]) / prof_steps}
     if workload in ("config2", "config3") and res["kernels"]["gjk_pairs_ms_per_step" if workload == "config2" else "convex_pairs_ms_per_step"] > 0:
         # secondary view: FP64 issue.  ~450 flop per GJK iteration on primitives (SURVEY 8d estimate; the
-        # convex kernels add 6 flop per hull vertex and support call); nominal B200 FP64 (non-tensor) 37 TFLOP/s
+        # convex kernels add 6 flop per hull vertex and support call); H100 SXM data sheet FP64 (non-tensor) 34 TFLOP/s
         it_flop = 450.0 if workload == "config2" else 450.0 + 2 * 64 * 6
         gsec = res["kernels"]["gjk_pairs_ms_per_step" if workload == "config2" else "convex_pairs_ms_per_step"] * 1e-3
         res["fp64_view"] = {"flop_per_gjk_iteration_estimate": it_flop,
                             "achieved_tflops_estimate": res["workload_stats"]["gjk_routed_pairs"] * res["workload_stats"]["gjk_iterations_mean"] * it_flop / gsec / 1e12,
-                            "nominal_fp64_tflops": 37.0}
+                            "nominal_fp64_tflops": 34.0}
     if workload == "config2":
         names = {P.GEOM_SPHERE: "sphere", P.GEOM_CAPSULE: "capsule", P.GEOM_BOX: "box", P.GEOM_CYLINDER: "cylinder"}
         t1, t2 = w["shapes"]["type"][w["h1"]], w["shapes"]["type"][w["h2"]]
         res["workload_stats"]["type_histogram"] = {"%s-%s" % (names[a], names[b]): int(((t1 == a) & (t2 == b)).sum())
                                                    for a in names for b in names}
     res["l2"] = ("L2 flushed between steps (256 MB overwrite inside the timed region)" if flush is not None else
-                 "inputs+outputs per step (%d MB) exceed the 126 MB L2; no explicit flush" % ((n * (BYTES_PER_PAIR - 80)) >> 20))
+                 "inputs+outputs per step (%d MB) exceed the 50 MB L2; no explicit flush" % ((n * (BYTES_PER_PAIR - 80)) >> 20))
     del eng
     return res
 
@@ -602,11 +619,18 @@ def measure_config5(args, rank, local, world, dist, steps, warmup, n_objects=Non
     barrier()
     e0.record()
     for k in range(steps):
-        acc["pairs"] += step(k)
+        last = step(k)
+        acc["pairs"] += last
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
     st1 = eng.stats()
+    if args.dump_outputs and n_objects is None:
+        # candidate pairs are appended in no fixed order: sorted by (first, second) so that runs compare row by row
+        f, s2 = d_f[:last].cpu().numpy(), d_s[:last].cpu().numpy()
+        recs = d_out[:last * P.contact_dtype.itemsize].cpu().numpy().view(P.contact_dtype)
+        order = np.lexsort((s2, f))
+        dump_records(args.dump_outputs, recs[order], {"first": f[order], "second": s2[order]})
     pairs = acc["pairs"]
     if world > 1:
         t = torch.tensor([ms], device="cuda", dtype=torch.float64)
@@ -751,7 +775,7 @@ def run_ours(args):
                     "warmup": max(args.warmup, 3), "ms_per_step": m["ms_per_step"], "higher_is_better": True,
                     "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
                     "config": {"workload": m["name"], "objects": m["n"], "env_scale": m["env_scale"],
-                               "l2": "poses, boxes, pairs and records of a step (%d MB) exceed the 126 MB L2" % (
+                               "l2": "poses, boxes, pairs and records of a step (%d MB) exceed the 50 MB L2" % (
                                    (m["n"] * 150 + int(m["candidate_pairs_per_step"]) * 350) >> 20),
                                "parallelism": "one scene over %d rank(s): every rank sweeps and collides the pairs of its own range of objects" % world},
                     "e2e": m["e2e"], "gpu_launches": m["gpu_launches"], "split_ms_per_step": m["split_ms_per_step"],

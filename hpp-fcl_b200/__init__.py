@@ -1,9 +1,9 @@
-"""hpp-fcl_b200 -- B200-native batched narrow-phase collision/distance engine.
+"""hpp-fcl_b200 -- batched narrow-phase collision/distance engine for the NVIDIA H100.
 
 Host-side mirror (Python) of the hpp-fcl query interface for the hot path
 collide()/distance() -> ShapeShapeDistance -> GJK/EPA (+ OBBRSS BVH traversal),
 on top of the C-ABI shared library built from csrc/ (include/hppfcl_b200.h).
-There is no CPU fallback: every query runs hand-written sm_100a CUDA kernels and
+There is no CPU fallback: every query runs hand-written sm_90a CUDA kernels and
 raises if the extension or a GPU is missing.
 """
 from . import _pod  # noqa: F401

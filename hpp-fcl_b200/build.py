@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA extension (sm_100a only) with nvcc.
+"""In-tree build of the CUDA extension (sm_90a only: H100) with nvcc.
 
 The product is a plain C-ABI shared library (include/hppfcl_b200.h): no torch
 types cross the boundary, so it is built with nvcc directly rather than through
@@ -12,8 +12,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_HERE, "csrc")
 _SO = os.path.join(_HERE, "libhppfcl_b200.so")
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+
+NVCC_FLAGS = GENCODE + [
     "-O3", "-std=c++17", "-lineinfo",
     # bit-exact parity with the FP64 reference semantics: no FMA contraction
     # (the oracle is compiled -ffp-contract=off); fp64 div/sqrt are IEEE already.
@@ -76,7 +77,7 @@ def build_extension(force=False, verbose=False):
     out = "".join(r[2] for r in results)
     rc = max(r[1] for r in results)
     if rc == 0:
-        cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC"] + ccbin + \
+        cmd = [_nvcc()] + GENCODE + ["-shared", "-Xcompiler", "-fPIC"] + ccbin + \
               ["-o", _SO] + [r[0] for r in results]
         res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         out += " ".join(cmd) + "\n" + res.stdout

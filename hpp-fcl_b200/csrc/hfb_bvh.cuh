@@ -1221,7 +1221,7 @@ HFB_HD void bvh_leaf(const BvhQuery& q, int primitive_id, const SolverP& P, EpaW
 // ---- warp-scheduled walk ------------------------------------------------------------------------
 // One lane walks one query's tree, depth first, in exactly the order of the reference's recursion.
 // Left to itself every lane of a warp would be in a different piece of code (bounding-volume test,
-// GJK on a leaf, EPA, stack handling) and queries differ tenfold in length: ncu showed 2.5 of 32 lanes
+// GJK on a leaf, EPA, stack handling) and queries differ tenfold in length: few lanes of a warp would be
 // active per issued instruction.  So (1) a lane that finishes a query fetches the next one itself, and
 // (2) the lanes vote: each is waiting to set up a query, to run a bounding-volume test or to run a
 // leaf test; the warp runs the phase most lanes wait for and the others sit that round out.  The order

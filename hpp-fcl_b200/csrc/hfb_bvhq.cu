@@ -7,10 +7,10 @@
 // bounding-volume phase every warp takes BV items until their queue is empty, then -- after a block barrier -- every
 // warp takes leaf items; the lane that completes a query's last outstanding item continues that query's walk
 // (q_advance), which pushes the next item(s) or retires the query and starts another.
-// Why phases and not "any warp takes any item" (the first version, profiles/r02_k_bvhq_*): the kernel is ~18 000
+// Why phases and not "any warp takes any item" (the first version): the kernel is ~18 000
 // instructions, the SM's instruction cache holds 2 000 (L1.5: 32 KB) -- with its eight warps in eight different
-// places of that code ncu showed 8.9 stall cycles per issued instruction waiting for instruction fetch.  In a
-// phase the eight warps run the same two thousand instructions at the same time.
+// places of that code the warps stall on instruction fetch.  In a phase the eight warps run the same two thousand
+// instructions at the same time.
 #include <cfloat>
 #include <type_traits>
 
@@ -325,7 +325,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_bvhq(const BvhqLaunch L) {
     // ---- bounding-volume phase: bv_gens generations of items.  A generation is what was queued when it started;
     // the items it pushes (a walk going down a level) are the next generation.  Running "until the queue is empty"
     // instead made every cycle wait for its deepest descent with a handful of lanes busy
-    // (profiles/r02_summary.md: 66 us of BV phase per cycle against 10 us of leaf phase). ----
+    // (BV phases of several times the length of the leaf phases). ----
     for (int gen = 0; gen < L.bv_gens; ++gen) {
       if (gen > 0) __syncthreads();
       if (threadIdx.x == 0) {

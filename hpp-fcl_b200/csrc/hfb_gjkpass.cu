@@ -2,8 +2,8 @@
 // PATH_GJKROUTE> on the GJK-routed classes; same per-pair operations: pair_gjk_begin / gjk_step / pair_gjk_end of
 // hfb_pair.cuh, i.e. GJK::evaluate src/narrowphase/gjk.cpp:188-370 and the extractors narrowphase.h:589-656).
 //
-// Why.  ncu on the single kernel (profiles/r01_ncu_k_pairs_gjkroute_raw.txt): 9 of 32 lanes active per instruction
-// and 6.9 stall cycles per issued instruction waiting for instruction fetch.  A pair needs 3 to 26 iterations, so
+// Why.  In the single kernel few lanes of a warp are active per instruction and the warps stall on instruction
+// fetch.  A pair needs 3 to 26 iterations, so
 // a warp that keeps its 32 pairs until the last one has converged idles most of its lanes; and set-up, iteration
 // and witness extraction together are ~13 000 instructions against an instruction cache of 2 000 (32 KB L1.5 per
 // SM), with the warps of an SM spread all over them.  Here:
@@ -12,7 +12,7 @@
 //                 (the last pass runs to convergence)
 //   k_gjk_end     status machine + witness points of every pair: result record, or an EPA queue item
 // Every kernel is small, and the later passes run full warps of the long pairs.  The state costs 424 B per pair
-// and pass of HBM traffic (0.5 M pairs: 0.2 GB, 0.04 ms at the measured bandwidth).
+// and pass of HBM traffic (0.5 M pairs: 0.2 GB).
 #include "hfb_gjkpass.h"
 
 #include <cub/cub.cuh>

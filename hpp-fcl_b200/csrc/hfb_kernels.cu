@@ -1,4 +1,4 @@
-// CUDA kernels (sm_100a) and the C-ABI of include/hppfcl_b200.h.
+// CUDA kernels (sm_90a) and the C-ABI of include/hppfcl_b200.h.
 //
 // Kernel inventory (DESIGN.md section 3 has the measurements)
 //   k_bin_hist/scan/scatter  device-side counting sort of the batch by pair class (closed-form combos |
@@ -13,7 +13,7 @@
 //                          reduced-size workspace, tier 1 retries the pairs that outgrew it
 //   k_bvh<MODE,KINDS,MINB> OBBRSS tree walks: mesh-shape (warp-scheduled, exact DFS order) and mesh-mesh
 //   k_convex_support       batched ConvexBase support argmax (warp per query, coalesced streaming of the
-//                          vertex block: HBM-bound, 77 % of the measured peak over a 1.2 GB pool)
+//                          vertex block: HBM-bound over a 1.2 GB pool)
 // MODE 0 = distance() epilogue, MODE 1 = collide() epilogue.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -37,9 +37,9 @@
 #include "hfb_broadphase.h"
 
 // lanes per pair: pairs touching ConvexBase/TriangleP (GC: 1, 2, 4, 8, 16, 32) and the EPA kernel
-// (GE: 4, 8, 16, 32).  The defaults are the measured optimum on B200 (profiles/r01_summary.md: the
-// scalar part of a GJK iteration is repeated by every lane of the group, so small groups win until
-// divergence between the pairs of a warp takes over at 1); HFB_GC / HFB_GE override them per context.
+// (GE: 4, 8, 16, 32).  Small groups are the defaults (the scalar part of a GJK iteration is repeated by
+// every lane of the group, so small groups win until divergence between the pairs of a warp takes over
+// at 1); HFB_GC / HFB_GE override them per context.
 #define HFB_GC_DEFAULT 2
 #define HFB_GE_DEFAULT 8
 
@@ -209,7 +209,7 @@ __global__ void __launch_bounds__(128, MINB) k_pairs(const BatchArgs a) {
 
 // Phase 1 for the GJK-routed primitive classes with lane refill.  GJK takes 3 to 26 iterations inside
 // one class; with a pair per lane for the whole kernel a warp runs at the pace of its slowest pair
-// (ncu: 9 of 32 lanes active per instruction).  Here a lane is in one of three states -- needs a pair,
+// (few lanes active per instruction).  Here a lane is in one of three states -- needs a pair,
 // iterating, needs its result extracted -- and the warp alternates between an iteration round (every
 // iterating lane does one GJK iteration) and a service round (finished lanes extract + store or queue
 // for EPA, then every free lane takes the next pair and sets it up).  Results do not depend on the
@@ -577,8 +577,7 @@ __global__ void k_bin_scan(const unsigned* hist, unsigned* offsets, unsigned* cu
 }
 // A block takes a window of HFB_SCATTER_ITEMS * 256 consecutive pairs: ranks inside the block by shared-memory
 // atomics, ONE global reservation per class and block, then the writes.  (The first form reserved per warp and class
-// through __match_any_sync + a global atomic: 300 k atomics on 49 addresses per 1 M pairs, 0.12 ms -- 8 % of a
-// config-2 step.)  A class's slice of the list is now made of runs of pairs from the same window, which also keeps the
+// through __match_any_sync + a global atomic: 300 k atomics on 49 addresses per 1 M pairs.)  A class's slice of the list is now made of runs of pairs from the same window, which also keeps the
 // gathers of the kernels that follow close together.
 #define HFB_SCATTER_ITEMS 8
 __global__ void __launch_bounds__(256) k_bin_scatter(const hfb_shape* shapes, uint32_t nshapes, const uint32_t* h1,
@@ -828,18 +827,18 @@ struct hfb_ctx {
   int bvhq = 1;        // HFB_BVHQ=0: mesh-shape distance queries through the lane-per-query kernel k_bvh instead of the task system k_bvhq
   // HFB_GJK_PASSES="6" (default) or e.g. "3,3,4": iterations of the first passes of the primitive-pair GJK (one more pass runs to
   // convergence); "0": the single kernel k_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE>
-  // iterations of the first pass; measured on config 2 (profiles/r02_summary.md), GJK kernels per 498 k pairs:
-  // "6" 1.10 ms, "8" 1.01, "9" 0.99, "10" 0.97, "12" 0.98, "16" 1.06, "10,10" 0.99, "4,4" 1.15; single kernel 1.16
+  // iterations of the first pass: 10 (a pass of few iterations leaves most pairs to the next; a long one idles the lanes
+  // of the pairs that converged early)
   int gjk_steps[8] = {10, 0, 0, 0, 0, 0, 0, 0};
   int gjk_npass = 2;
   // HFB_EPA_OVERLAP=1: EPA of the pairs the first GJK pass finished starts on a side stream next to the remaining passes;
-  // measured slower on config 2 (2.11 vs 2.00 ms per step: the two kernels take each other's SMs), so off
+  // off by default: the two kernels take each other's SMs
   int epa_overlap = 0;
   int bvh_warps = 8;   // HFB_BVH_WARPS: 8 (255 registers per thread) or 16 (128) warps per block of k_bvhq
   int bvh_gens = 2;    // HFB_BVH_GENS: generations of BV items per cycle of k_bvhq
   int bvh_spec_big = 300;  // HFB_BVH_SPEC_BIG: items more before subtrees of up to 128 triangles are speculated
   int hull_sort = 1;      // HFB_HULL_SORT: second sort key (first operand's handle) inside the hull / triangle class
-  int gjk_ordered = 0;    // HFB_GJK_ORDERED=1: the second GJK pass takes the survivors of the first in class order (measured: no gain)
+  int gjk_ordered = 0;    // HFB_GJK_ORDERED=1: the second GJK pass takes the survivors of the first in class order (off by default)
   int epa_resume = 8192;  // HFB_EPA_RESUME: retries per batch that continue from the state tier 0 reached (5 KB each)
   int bvh_chunk = 6;   // HFB_BVH_GJK_CHUNK: GJK iterations a leaf item runs before it parks its state
   int bvh_spec = 200;  // HFB_BVH_SPEC: items a query uses before it may speculate on subtrees (< 0: never)
@@ -1096,8 +1095,8 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
   av.range_hi = offsets + HFB_BIN_BVH;
   if ((rc = launch_pairs<1, CAP_PRIM | CAP_PLANE, MODE, PATH_CLOSED>(ctx, ac, n, s))) return rc;
   // the class populations are only known on the device, so both GJK ranges are cut the same way
-  // measured on B200 (profiles/r01_summary.md): cutting phase 1 costs more in kernel tails than the overlap
-  // returns, so one part is the default; HFB_NSUB asks for more
+  // cutting phase 1 costs more in kernel tails than the overlap returns, so one part is the default; HFB_NSUB asks
+  // for more
   unsigned nsub = ctx->nsub > 0 ? (unsigned)ctx->nsub : 1u;
   if (!want_epa) nsub = 1;
   if (nsub > (unsigned)(kMaxParts / 2)) nsub = kMaxParts / 2;
@@ -1345,9 +1344,9 @@ int host_batch_pipelined(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_t
   auto stamp = [&](const char* what) {
     if (trace) fprintf(stderr, "[hfb pipe] %-28s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
   };
-  // How many chunks: a chunk's phase 1 has a floor of ~0.25 ms whatever its size (the serial iteration chains of the
-  // longest pairs in the GJK passes), so chunks are only worth their overlap: about one per 0.6 ms of PCIe time
-  // (uploads and downloads share the link, ~57 GB/s measured), at least 128 Ki pairs each.  1 M pairs: a scene +
+  // How many chunks: a chunk's phase 1 has a floor whatever its size (the serial iteration chains of the longest pairs
+  // in the GJK passes), so chunks are only worth their overlap: about one per 0.6 ms of PCIe time (uploads and
+  // downloads share the link), at least 128 Ki pairs each.  1 M pairs: a scene +
   // distances only (16 B per pair) -> 1 chunk; a scene + full rows (104 B) -> 3; pair rows + full rows (296 B) -> 8.
   size_t chunk;
   if (ctx->chunk > 0) {
@@ -1444,7 +1443,7 @@ int host_batch_pipelined(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_t
     if (min_out) CK(cudaMemcpyAsync(min_out + done, static_cast<double*>(ctx->big_min.p) + done, m * 8, cudaMemcpyDeviceToHost, sD));
     else CK(cudaMemcpyAsync(out + done, d_out + done, m * sizeof(OutT), cudaMemcpyDeviceToHost, sD));
     // the chunk's handles / object indices are validated AFTER its work is enqueued, while the GPU is busy with it (8 MB
-    // of host reads per 1 M pairs: 0.4 ms in front of a single-chunk call otherwise).  The device side is safe against
+    // of host reads per 1 M pairs, in front of a single-chunk call otherwise).  The device side is safe against
     // a bad value (k_expand_pairs, handle_type, load_shape: such a pair comes back unsupported); the call fails.
     if (obj) {
       const uint32_t no = (uint32_t)(obj->n_objects > 0xffffffffull ? 0xffffffffull : obj->n_objects);
@@ -1559,8 +1558,8 @@ int host_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform* 
   const int32_t* hin = cached ? req->q.cached_support_func_guess : nullptr;
   {  // large plain batches: phase 1 chunk by chunk, EPA once (host_batch_pipelined)
     const bool plain = !go && !extra_out && !counts_out && !(om && om->flags) && !gin && !hin;
-    // (full records only: with 8 bytes per pair down there is nothing to overlap and the rotating slots are as fast --
-    // measured 4.2e8 against 4.4e8 pairs/s; HFB_HOST_PIPE=2 sends those calls here as well)
+    // (full records only: with 8 bytes per pair down there is nothing to overlap and the rotating slots serve;
+    // HFB_HOST_PIPE=2 sends those calls here as well)
     const bool min_only = om && om->min_out;
     bool take = ctx->host_pipe && plain && n >= kChunk && n <= (size_t)16 << 20 && (min_only ? ctx->host_pipe > 1 : out != nullptr);
     if (take && ctx->host_pipe < 2 && ctx->pipe_epa_frac > 1.0 / 16 && ++ctx->pipe_skipped % 16 != 0) take = false;
@@ -1573,8 +1572,8 @@ int host_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform* 
   }
   size_t done = 0;
   int si = 0;
-  // object-table calls send 8 B per pair up: fewer, larger chunks (measured: 256 Ki pairs 2.57 ms per 1 M pairs with
-  // 8-byte results against 3.00 ms at 128 Ki); the row form is bound by its 200 B per pair of H2D and pipelines best at 128 Ki
+  // object-table calls send 8 B per pair up: fewer, larger chunks (256 Ki); the row form is bound by its 200 B per pair
+  // of H2D and takes 128 Ki
   size_t chunk = ctx->chunk > 0 ? (size_t)ctx->chunk : (obj ? 2 * kChunk : kChunk);
   chunk = (chunk + 31) & ~(size_t)31;  // the compact collide mode writes whole 32-pair flag words per chunk
   unsigned* d_hits = nullptr;
@@ -1756,7 +1755,7 @@ int device_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform
 // ==================================================================== C-ABI ===
 extern "C" {
 
-const char* hfb_version(void) { return "hppfcl_b200 0.1 (sm_100a, fp64, fmad=false)"; }
+const char* hfb_version(void) { return "hppfcl_b200 0.1 (sm_90a, fp64, fmad=false)"; }
 
 void hfb_default_distance_request(hfb_distance_request* r) {
   std::memset(r, 0, sizeof(*r));

@@ -13,8 +13,7 @@
 #define HFB_HD __host__ __device__ __forceinline__
 #define HFB_D __device__ __forceinline__
 // out-of-line on the device: multi-call-site helpers that run once per pair; inlining
-// them multiplies the kernel's code size (instruction-cache misses dominated the first
-// ncu profile of k_pairs: stall_no_instruction 9.7 cycles per issue)
+// them multiplies the kernel's code size (instruction-cache misses then dominate k_pairs)
 #define HFB_HD_NOINLINE __host__ __device__ __noinline__ inline
 #else
 #define HFB_HD inline

@@ -174,7 +174,7 @@ HFB_HD v3 prim_support_inl(int type, double p0, double p1, double p2, v3 dir) {
 }
 // primitive supports, out of line on the device: one copy of this code serves both operands of
 // the Minkowski difference (inlined twice it dominated the GJK loop's instruction footprint and the
-// kernel stalled on instruction fetch, see profiles/r01_summary.md)
+// kernel stalled on instruction fetch)
 HFB_HD_NOINLINE v3 prim_support(int type, double p0, double p1, double p2, v3 dir) {
   return prim_support_inl(type, p0, p1, p2, dir);
 }

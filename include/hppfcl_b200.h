@@ -1,5 +1,5 @@
 /*
- * hppfcl_b200.h -- C-ABI of the B200-native batched narrow-phase engine.
+ * hppfcl_b200.h -- C-ABI of the batched narrow-phase engine (CUDA, NVIDIA H100).
  *
  * This is the drop-in boundary for the hot path of hpp-fcl
  * (collide()/distance() -> ShapeShapeDistance -> GJKSolver::shapeDistance ->

@@ -6,7 +6,7 @@ reports to its collision callback."""
 import numpy as np
 import pytest
 
-from tests.common import P, hf
+from tests.common import P, hf, reference_scene
 from hppfcl_b200 import workloads as W
 
 
@@ -76,13 +76,10 @@ def test_scene_boxes_equal_the_reference():
     bit, poses with and without rotation"""
     import os
     from oracle import oracle_lib
-    from tests.common import EmuScene
-    if os.path.isdir("/root/reference/src"):
-        oracle_lib.build_ref()
-    if not oracle_lib.ref_available():
-        pytest.skip("oracle/_ref is not built (needs /root/reference)")
+    from tests.common import EmuScene, reference_scene
+    oracle_lib.build_ref()
     rng = np.random.default_rng(12)
-    ref, emu = oracle_lib.RefScene(P), EmuScene()
+    ref, emu = reference_scene(), EmuScene()
     prims = W.random_primitive_shapes(rng, 48, (P.GEOM_BOX, P.GEOM_SPHERE, P.GEOM_CAPSULE, P.GEOM_CYLINDER, P.GEOM_CONE,
                                                 P.GEOM_ELLIPSOID))
     prims["ssr"] = np.where(rng.random(48) < 0.3, 0.05, 0.0)
@@ -222,11 +219,11 @@ def test_scene_with_a_floor_and_a_wall():
     tf["T"][:400, 2] = rng.uniform(-0.3, 0.6, 400)  # four hundred objects on or in the floor
     tf["T"][0] = 0
     bb = eng.scene_aabbs(oh, tf)
-    if oracle_lib.ref_available():
-        ref = oracle_lib.RefScene(P)
-        assert np.array_equal(np.concatenate([ref.register_shapes(prims), ref.register_halfspaces(P.GEOM_HALFSPACE, nd_floor),
-                                              ref.register_halfspaces(P.GEOM_PLANE, nd_wall)]), hs[0])
-        assert np.array_equal(ref.object_aabbs(oh, tf), bb)
+    oracle_lib.build_ref()
+    ref = reference_scene()
+    assert np.array_equal(np.concatenate([ref.register_shapes(prims), ref.register_halfspaces(P.GEOM_HALFSPACE, nd_floor),
+                                          ref.register_halfspaces(P.GEOM_PLANE, nd_wall)]), hs[0])
+    assert np.array_equal(ref.object_aabbs(oh, tf), bb)
     f, s = hf.broadphase_pairs(bb)
     want = set(zip(f.tolist(), s.tolist()))
     assert sum(1 for a, b in want if a == 0) > 150 and sum(1 for a, b in want if b == n - 1) > 20

@@ -306,11 +306,12 @@ def _contacts_scene(backends):
     meshes = [W.sphere_mesh(1.0, 20, 10, noise=0.03, rng=rng), W.sphere_mesh(0.6, 12, 6, noise=0.05, rng=rng)]
     from oracle import oracle_lib
     from hppfcl_b200.engine import build_bvh_obbrss
+    from tests.common import ReferenceScene
     ids = []
     for v, t in meshes:
         got = set()
         for s in backends.values():
-            if isinstance(s, oracle_lib.OracleScene):
+            if isinstance(s, (oracle_lib.OracleScene, ReferenceScene)):  # (they build the tree themselves)
                 got.add(int(s.register_bvh(v, t)[0]))
             else:
                 got.add(int(s.register_bvh_obbrss(build_bvh_obbrss(v, t), v, t)))
@@ -374,13 +375,9 @@ def _check_contacts(backends, h1, tf1, h2, tf2, first, others):
 
 def test_all_contacts_of_mesh_pairs():
     from oracle import oracle_lib
-    from tests.common import EmuScene
-    import os
-    b = {"oracle": oracle_lib.OracleScene(P), "emu": EmuScene()}
-    if os.path.isdir("/root/reference/src"):
-        oracle_lib.build_ref()
-    if oracle_lib.ref_available():
-        b["ref"] = oracle_lib.RefScene(P)
+    from tests.common import EmuScene, reference_scene
+    oracle_lib.build_ref()
+    b = {"oracle": oracle_lib.OracleScene(P), "emu": EmuScene(), "ref": reference_scene()}
     h1, tf1, h2, tf2 = _contacts_scene(b)
     _check_contacts(b, h1, tf1, h2, tf2, "oracle", [k for k in b if k != "oracle"])
 

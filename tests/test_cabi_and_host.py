@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol(built):
     assert len(syms) >= 20
     for s in syms:
         assert hasattr(L, s), "missing export %s" % s
-    assert b"sm_100a" in L.hfb_version()
+    assert b"sm_90a" in L.hfb_version()
 
 
 def test_pod_layouts_match_header(built):

@@ -5,13 +5,13 @@ halfspace / halfspace-plane pairs (parallel, anti-parallel, crossing), distance(
 
   reference (oracle/_ref, /root/reference compiled in place)  ==  oracle          (CPU, where _ref exists)
   host build of the device code (tests/emu)                   ==  oracle          (CPU)
-  CUDA kernels through the C-ABI                              ==  oracle          (B200)
+  CUDA kernels through the C-ABI                              ==  oracle          (GPU)
 bit for bit (compare_distance(exact=True): status words, distances, witness points, normals).
 """
 import numpy as np
 import pytest
 
-from tests.common import P, compare_distance, make_scenes, EmuScene
+from tests.common import P, compare_distance, make_scenes, EmuScene, reference_scene
 from hppfcl_b200 import workloads as W
 from oracle import oracle_lib
 
@@ -106,12 +106,9 @@ def check(ref_out, got_out, what):
 
 def test_oracle_equals_the_reference():
     import os
-    if os.path.isdir("/root/reference/src"):
-        oracle_lib.build_ref()
-    if not oracle_lib.ref_available():
-        pytest.skip("oracle/_ref is not built (needs /root/reference)")
+    oracle_lib.build_ref()
     w = plane_world()
-    orc, ref = oracle_lib.OracleScene(P), oracle_lib.RefScene(P)
+    orc, ref = oracle_lib.OracleScene(P), reference_scene()
     ho = register(orc, w, "oracle")
     hr = register(ref, w, "ref")
     for x, y in zip(ho, hr):

@@ -1,13 +1,14 @@
-"""The oracle against THE REFERENCE ITSELF: oracle/_ref/libhppfcl_ref.so is /root/reference compiled in
+"""The oracle against THE REFERENCE ITSELF: oracle/_ref/libhppfcl_ref.so is the reference's sources compiled in
 place, unmodified (recipe: `make -C oracle ref`; Eigen/Boost stand-ins under oracle/ref_shim/).  The
 oracle's restatement must reproduce the reference's own collide()/distance() bit for bit: status words,
 iteration counts, distances, witness points, normals, contact ids, and the OBBRSS tree its builder makes.
-On the GPU box the same library (it travels with the snapshot) is the yardstick for the CUDA path.
+The same library is the yardstick for the CUDA path.  Where it is not built, the reference's recorded outputs
+answer (tests.common.reference_scene, tests/golden/reference_outputs.json.gz).
 """
 import numpy as np
 import pytest
 
-from tests.common import P, compare_distance
+from tests.common import P, compare_distance, reference_scene
 from hppfcl_b200 import workloads as W
 from oracle import oracle_lib
 
@@ -17,15 +18,12 @@ ALL = (P.GEOM_SPHERE, P.GEOM_CAPSULE, P.GEOM_BOX, P.GEOM_CYLINDER, P.GEOM_CONE, 
 @pytest.fixture(scope="module")
 def have_ref():
     import os
-    if os.path.isdir("/root/reference/src"):
-        oracle_lib.build_ref()
-    if not oracle_lib.ref_available():
-        pytest.skip("oracle/_ref is not built (needs /root/reference)")
+    oracle_lib.build_ref()
     return True
 
 
 def scenes():
-    return oracle_lib.OracleScene(P), oracle_lib.RefScene(P)
+    return oracle_lib.OracleScene(P), reference_scene()
 
 
 def cmp_collide(ref, got, what=""):
@@ -205,7 +203,7 @@ def test_gpu_against_the_reference_build(have_ref):
     import hppfcl_b200 as hf
     n = 200_000
     w = W.config2_mixed_primitives(n, pool=4096, types=ALL, seed=9)
-    ref = oracle_lib.RefScene(P)
+    ref = reference_scene()
     eng = hf.Engine(0)
     h = eng.register_shapes(w["shapes"])
     ref.register_shapes(w["shapes"])
@@ -218,7 +216,7 @@ def test_gpu_against_the_reference_build(have_ref):
                 eng.batch_collide(h[w["h1"]], w["tf1"], h[w["h2"]], w["tf2"]))
     # mesh vs shapes and mesh vs mesh, tree built by the product's host builder
     rng = np.random.default_rng(5)
-    eng2, ref2 = hf.Engine(0), oracle_lib.RefScene(P)
+    eng2, ref2 = hf.Engine(0), reference_scene()
     va, ta = W.sphere_mesh(1.0, 30, 15, noise=0.02, rng=rng)
     bid = eng2.register_bvh_obbrss(None, va, ta)
     rbid, _ = ref2.register_bvh(va, ta)
@@ -248,9 +246,7 @@ def test_plain_obb_models(have_ref):
     host build of the device code.  distance() on a plain OBB model is not offered (unsupported records)."""
     from tests.common import EmuScene
     orc, ref, hm, hp, rng, (na, rna, nb, rnb), ((va, ta), (vb, tb)) = mesh_scene()
-    L = oracle_lib.ref_lib()
-    L.ref_bvh_obb_is_obbrss_half.argtypes = [__import__("ctypes").c_void_p, __import__("ctypes").c_int]
-    assert L.ref_bvh_obb_is_obbrss_half(ref.h, 0) == 1 and L.ref_bvh_obb_is_obbrss_half(ref.h, 1) == 1
+    assert ref.obb_is_obbrss_half(0) == 1 and ref.obb_is_obbrss_half(1) == 1
     emu = EmuScene()
     assert emu.register_bvh_obbrss(na, va, ta) == 0 and emu.register_bvh_obbrss(nb, vb, tb) == 1
     # the same two meshes once more, as plain OBB models (ids 2 and 3 in every backend)

@@ -75,9 +75,11 @@ _prof = (_C.c_ulonglong * 5)()
 eng.L.hfb_debug_bvh_profile.argtypes = [_C.c_void_p, _C.c_void_p]
 eng.L.hfb_debug_bvh_profile(eng.h, _prof)
 _calls = steps + 3
-_nb = min(148, (n + 63) // 64)
-phase = {"bv_us_per_block": _prof[0] / 1.9e3 / _nb / _calls, "leaf_us_per_block": _prof[1] / 1.9e3 / _nb / _calls,
-         "epa_us_per_block": _prof[2] / 1.9e3 / _nb / _calls, "cycles_per_block": _prof[3] / _nb / _calls,
+# k_bvhq runs at most one block per SM (bvhq_blocks); the counters are SM clock cycles
+_nb = min(torch.cuda.get_device_properties(0).multi_processor_count, (n + 63) // 64)
+_cyc_per_us = torch.cuda.clock_rate(0)  # current SM clock, MHz
+phase = {"bv_us_per_block": _prof[0] / _cyc_per_us / _nb / _calls, "leaf_us_per_block": _prof[1] / _cyc_per_us / _nb / _calls,
+         "epa_us_per_block": _prof[2] / _cyc_per_us / _nb / _calls, "cycles_per_block": _prof[3] / _nb / _calls,
          "epa_phases_per_block": _prof[4] / _nb / _calls}
 print(json.dumps({"phase_profile": phase, "workload": "config4: 10k-tri OBBRSS mesh vs %d capsules, distance" % n, "queries_per_s": n / (ms * 1e-3),
                   "ms_per_batch": ms, "k_bvh_ms": kt["bvh_ms"] / steps, "host_api_queries_per_s": n / t_host,

@@ -18,7 +18,7 @@ import time
 import numpy as np
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "..", ".."))
-from tests.common import P, EmuScene, compare_distance  # noqa: E402
+from tests.common import P, EmuScene, compare_distance, reference_scene  # noqa: E402
 from hppfcl_b200 import workloads as W  # noqa: E402
 from oracle import oracle_lib  # noqa: E402
 
@@ -210,7 +210,7 @@ class Backends:
 
     def __init__(self, use_ref, use_emu):
         self.orc = oracle_lib.OracleScene(P)
-        self.ref = oracle_lib.RefScene(P) if use_ref else None
+        self.ref = reference_scene() if use_ref else None
         self.emu = (use_emu if not isinstance(use_emu, bool) else EmuScene()) if use_emu else None
 
     def register_shapes(self, s):
@@ -556,9 +556,8 @@ def main():
     CONTACTS[0] = a.contacts
     PLANES[0] = a.planes
     DRIFT[0] = a.drift
-    if os.path.isdir("/root/reference/src"):
-        oracle_lib.build_ref()
-    use_ref = oracle_lib.ref_available()
+    oracle_lib.build_ref()
+    use_ref = oracle_lib.ref_available()  # (arbitrary seeds: only the reference build itself can answer)
     t0, seed, bad = time.time(), a.seed, 0
     while time.time() - t0 < a.minutes * 60:
         dev = not a.no_emu

@@ -1,4 +1,4 @@
-"""Digest of an ncu report for profiles/: the launch's key raw metrics, stall reasons per issued instruction, and the
+"""Digest of an ncu report: the launch's key raw metrics, stall reasons per issued instruction, and the
 source lines (CUDA view, needs -lineinfo + --import-source on) that carry most stall samples / instructions.
   python tests/tools/ncu_digest.py report.ncu-rep [out.txt]      (runs `ncu -i`, so it works on the GPU box, where a
 report of the big kernels is too large to bring back)"""
