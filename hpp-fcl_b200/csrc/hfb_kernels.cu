@@ -781,6 +781,11 @@ struct Slot {
   cudaStream_t epa_stream = nullptr;
   cudaEvent_t ev_part[kMaxParts] = {};
   cudaEvent_t ev_join = nullptr;
+  // GJK passes, the hull / triangle kernel and EPA of a batch run here, at the device's highest stream priority, next
+  // to the closed forms on the caller's stream: the block scheduler gives free SMs to the long GJK / EPA chains first
+  // and the closed-form blocks fill the tails.  ev_fork / ev_work: the fork after the class sort and the join.
+  cudaStream_t work_stream = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_work = nullptr;
   DevBuf cont;  // EpaCont records (k_epa tier 0 -> tier 1)
   DevBuf h1, h2, tf1, tf2, out, gin, hin, gout, hout, queue, counters, lists, retry, bvh_ws, bvh_cnt, extra, ccnt, okeys, ohist, olist;
   DevBuf qprep, qstacks, qtl, qws, qsv;  // task-system mesh-shape walk (hfb_bvhq.cu)
@@ -996,6 +1001,11 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
     CK(cudaStreamCreateWithFlags(&sl.epa_stream, cudaStreamNonBlocking));
     for (int k = 0; k < kMaxParts; ++k) CK(cudaEventCreateWithFlags(&sl.ev_part[k], cudaEventDisableTiming));
     CK(cudaEventCreateWithFlags(&sl.ev_join, cudaEventDisableTiming));
+    int least = 0, greatest = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    CK(cudaStreamCreateWithPriority(&sl.work_stream, cudaStreamNonBlocking, greatest));
+    CK(cudaEventCreateWithFlags(&sl.ev_fork, cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&sl.ev_work, cudaEventDisableTiming));
   }
   CK(sl.lists.reserve((size_t)n * sizeof(uint32_t)));
   CK(sl.retry.reserve((size_t)n * sizeof(uint32_t)));
@@ -1055,6 +1065,11 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
     a.index_list = sorted;
   }
   const bool want_epa = a.P.compute_penetration;
+  // fork: GJK, the hull / triangle kernel and EPA on the work stream; the closed forms (nothing reads their rows) and
+  // the mesh walks stay on the caller's stream, which waits for the work stream before the batch returns
+  cudaStream_t ws = sl.work_stream;
+  CK(cudaEventRecord(sl.ev_fork, s));
+  CK(cudaStreamWaitEvent(ws, sl.ev_fork, 0));
 
   // EPA over the queue items pushed since the previous mark.  Parts other than the last go to the
   // side stream, where they overlap phase 1 of the parts that follow; an EPA item is long and there
@@ -1063,27 +1078,27 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
   auto epa_after_part = [&](bool last) -> int {
     if (!want_epa || epa_mode) return HFB_OK;
     const int j = parts_done++;
-    if (cudaMemcpyAsync(mark + j + 1, cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s) != cudaSuccess)
+    if (cudaMemcpyAsync(mark + j + 1, cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, ws) != cudaSuccess)
       return fail(ctx, HFB_ERR_CUDA, "queue mark copy failed");
     BatchArgs ae = a;
     ae.epa_lo = mark + j;
     ae.epa_hi = mark + j + 1;
     ae.epa_head = heads + j;
-    cudaStream_t es = s;
+    cudaStream_t es = ws;
     if (!last) {
       es = sl.epa_stream;
-      if (cudaEventRecord(sl.ev_part[j], s) != cudaSuccess || cudaStreamWaitEvent(es, sl.ev_part[j], 0) != cudaSuccess)
+      if (cudaEventRecord(sl.ev_part[j], ws) != cudaSuccess || cudaStreamWaitEvent(es, sl.ev_part[j], 0) != cudaSuccess)
         return fail(ctx, HFB_ERR_CUDA, "event record/wait failed");
     } else if (j > 0) {
       // the side stream's launches finish before the caller's stream moves past this batch
-      if (cudaEventRecord(sl.ev_join, sl.epa_stream) != cudaSuccess || cudaStreamWaitEvent(s, sl.ev_join, 0) != cudaSuccess)
+      if (cudaEventRecord(sl.ev_join, sl.epa_stream) != cudaSuccess || cudaStreamWaitEvent(ws, sl.ev_join, 0) != cudaSuccess)
         return fail(ctx, HFB_ERR_CUDA, "event record/wait failed");
     }
     int r = mixed ? launch_epa_g<CAPS_ALL, MODE, 0>(ctx, ae, es) : launch_epa_g<CAP_PRIM, MODE, 0>(ctx, ae, es);
     if (r || !last) return r;
     // tier 1 over the retry list, after every tier-0 launch of this batch
     ae.epa_head = cnt + 3;
-    return mixed ? launch_epa_g<CAPS_ALL, MODE, 1>(ctx, ae, s) : launch_epa_g<CAP_PRIM, MODE, 1>(ctx, ae, s);
+    return mixed ? launch_epa_g<CAPS_ALL, MODE, 1>(ctx, ae, ws) : launch_epa_g<CAP_PRIM, MODE, 1>(ctx, ae, ws);
   };
 
   BatchArgs ac = a, ag = a, av = a;
@@ -1105,16 +1120,16 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
     ag.sub_idx = j;
     ag.sub_cnt = nsub;
     switch (ctx->minb) {  // register budget of the GJK kernel: 255 / 168 / 128 registers per thread
-      case 3: rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 3>(ctx, ag, sub_work, s); break;
-      case 4: rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 4>(ctx, ag, sub_work, s); break;
+      case 3: rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 3>(ctx, ag, sub_work, ws); break;
+      case 4: rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 4>(ctx, ag, sub_work, ws); break;
       default:
         if (ctx->refill) {
           ag.gjk_work = cnt + 26 + j;
           ag.iter_quorum = (unsigned)ctx->iter_quorum;
           const unsigned blocks = (unsigned)ctx->num_sms * 2u;  // 255 registers: 2 blocks of 128 per SM
           {
-            KTimer kt(ctx, s, 0);
-            k_gjk_refill<MODE><<<blocks, 128, 0, s>>>(ag);
+            KTimer kt(ctx, ws, 0);
+            k_gjk_refill<MODE><<<blocks, 128, 0, ws>>>(ag);
           }
           ctx->stats.kernel_launches++;
           if (cudaGetLastError() != cudaSuccess) return fail(ctx, HFB_ERR_CUDA, "k_gjk_refill launch failed");
@@ -1128,24 +1143,24 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
           uint32_t* la = static_cast<uint32_t*>(sl.glist.p);
           const bool early_epa = ctx->gjk_npass > 1 && ctx->epa_overlap && want_epa;
           {
-            KTimer kt(ctx, s, 0);
+            KTimer kt(ctx, ws, 0);
             if (gjk_passes_first(ag, MODE, n, sl.gstate.p, la, static_cast<unsigned*>(sl.gcnt.p), ctx->gjk_steps, ctx->gjk_npass,
-                                 ctx->num_sms, s, &nl, ctx->gjk_ordered ? sl.gsel.p : nullptr, early_epa) != 0)
+                                 ctx->num_sms, ws, &nl, ctx->gjk_ordered ? sl.gsel.p : nullptr, early_epa) != 0)
               return fail(ctx, HFB_ERR_CUDA, "GJK pass launch failed");
           }
           // EPA of the pairs the first pass finished starts on the side stream, next to the remaining passes (which
           // only keep a fraction of the GPU busy)
           if (early_epa && (rc = epa_after_part(false))) return rc;
           {
-            KTimer kt(ctx, s, 0);
+            KTimer kt(ctx, ws, 0);
             if (gjk_passes_rest(ag, MODE, n, sl.gstate.p, la, la + n, static_cast<unsigned*>(sl.gcnt.p), ctx->gjk_steps,
-                                ctx->gjk_npass, ctx->num_sms, s, &nl, early_epa) != 0)
+                                ctx->gjk_npass, ctx->num_sms, ws, &nl, early_epa) != 0)
               return fail(ctx, HFB_ERR_CUDA, "GJK pass launch failed");
           }
           ctx->stats.kernel_launches += (uint64_t)nl;
           rc = HFB_OK;
         } else {
-          rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 1>(ctx, ag, sub_work, s);
+          rc = launch_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE, 1>(ctx, ag, sub_work, ws);
         }
     }
     if (rc) return rc;
@@ -1155,7 +1170,7 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
     for (unsigned j = 0; j < nsub; ++j) {
       av.sub_idx = j;
       av.sub_cnt = nsub;
-      if ((rc = launch_pairs_convex<MODE>(ctx, av, sub_work, s))) return rc;
+      if ((rc = launch_pairs_convex<MODE>(ctx, av, sub_work, ws))) return rc;
       if ((rc = epa_after_part(j + 1 == nsub))) return rc;
     }
   }
@@ -1256,6 +1271,8 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
       CK(cudaGetLastError());
     }
   }
+  CK(cudaEventRecord(sl.ev_work, ws));
+  CK(cudaStreamWaitEvent(s, sl.ev_work, 0));
   ctx->stats.pairs_processed += n;
   return HFB_OK;
 }
@@ -1861,9 +1878,12 @@ void hfb_ctx_destroy(hfb_ctx* c) {
     for (DevBuf* b : bs) b->release();
     if (s.stream) cudaStreamDestroy(s.stream);
     if (s.epa_stream) cudaStreamDestroy(s.epa_stream);
+    if (s.work_stream) cudaStreamDestroy(s.work_stream);
     for (cudaEvent_t e : s.ev_part)
       if (e) cudaEventDestroy(e);
     if (s.ev_join) cudaEventDestroy(s.ev_join);
+    if (s.ev_fork) cudaEventDestroy(s.ev_fork);
+    if (s.ev_work) cudaEventDestroy(s.ev_work);
   };
   for (int k = 0; k < kSlots; ++k) rel(c->slots[k]);
   rel(c->dev_slot);
