@@ -540,9 +540,9 @@ HFB_HD_NOINLINE Param4 proj_tetra_origin(v3 a, v3 b, v3 c, v3 d) {
   return res;
 }
 
-// details::getClosestPoints (gjk.cpp:94-151) on a by-value simplex
-HFB_HD_NOINLINE void closest_points(const SV& v0, const SV& v1, const SV& v2, const SV& v3_, int rank, v3& w0,
-                           v3& w1) {
+// details::getClosestPoints (gjk.cpp:94-151) on a by-value simplex.  Most kernels call it out of line (closest_points);
+// one that inlines it keeps the simplex in registers (passed by reference to the call, it goes to local memory).
+HFB_HD void closest_points_inl(const SV& v0, const SV& v1, const SV& v2, const SV& v3_, int rank, v3& w0, v3& w1) {
   if (rank == 1) {
     w0 = v0.w0;
     w1 = v0.w1;
@@ -584,6 +584,10 @@ HFB_HD_NOINLINE void closest_points(const SV& v0, const SV& v1, const SV& v2, co
     w1 = w1 + pr.p3 * v3_.w1;
   }
 }
+HFB_HD_NOINLINE void closest_points(const SV& v0, const SV& v1, const SV& v2, const SV& v3_, int rank, v3& w0,
+                                   v3& w1) {
+  closest_points_inl(v0, v1, v2, v3_, rank, w0, w1);
+}
 
 // details::inflate (gjk.cpp:158-173)
 HFB_HD void inflate(const MinkD& md, v3 normal, v3& w0, v3& w1) {
@@ -591,9 +595,11 @@ HFB_HD void inflate(const MinkD& md, v3 normal, v3& w0, v3& w1) {
   if (md.ssr1 > 0) w1 = w1 - md.ssr1 * normal;
 }
 
-// GJK::getWitnessPointsAndNormal (gjk.cpp:177-186)
+// GJK::getWitnessPointsAndNormal (gjk.cpp:177-186); INL: closest_points inlined
+template <bool INL = false>
 HFB_HD void gjk_witness(const GjkState& g, const MinkD& md, v3& w0, v3& w1, v3& normal) {
-  closest_points(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1);
+  if (INL) closest_points_inl(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1);
+  else closest_points(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1);
   if (nrm(w1 - w0) > HFB_DUMMY_PRECISION) normal = unit(w1 - w0);
   else normal = -unit(g.ray);
   inflate(md, normal, w0, w1);

@@ -7,73 +7,213 @@
 // a warp that keeps its 32 pairs until the last one has converged idles most of its lanes; and set-up, iteration
 // and witness extraction together are ~13 000 instructions against an instruction cache of 2 000 (32 KB L1.5 per
 // SM), with the warps of an SM spread all over them.  Here:
-//   k_gjk_first   set-up + the first K1 iterations of every pair            -> solver state (GjkSaved) to HBM
+//   k_gjk_first   set-up + the first K1 iterations of every pair            -> finished-pair or loop state to HBM
 //   k_gjk_more    K2, K3, ... more iterations of the pairs still running, which each pass compacts into a list
 //                 (the last pass runs to convergence)
 //   k_gjk_end     status machine + witness points of every pair: result record, or an EPA queue item
-// Every kernel is small, and the later passes run full warps of the long pairs.  The state costs 424 B per pair
-// and pass of HBM traffic (0.5 M pairs: 0.2 GB).
+// Every kernel is small, and the later passes run full warps of the long pairs.
+//
+// The state between the kernels is stored field-major (one row per scalar field, one column per pair), so that the
+// lanes of a warp, which hold consecutive pairs, move consecutive words.  A finished pair leaves 52 B plus 48 B per
+// live simplex vertex (w = w0 - w1 is not stored: gjk_support computed it that way); a pair still running leaves its
+// loop state, 56 B plus 48 B per live vertex (plus 52 B for the Polyak and Nesterov variants), at its slot in the
+// list of running pairs, where the next pass reads it densely.
 #include "hfb_gjkpass.h"
-
-#include <cub/cub.cuh>
 
 namespace {
 
-// (16-byte aligned: 432 B = 27 x 16, so that the copies to and from HBM can move 16 bytes per instruction)
-struct __align__(16) GjkSaved {
-  GjkState g;
-  GjkLoop L;
-  int done;  // 1: converged in the first pass (extracted early, so that its EPA can start), 2: in a later pass, 0: running
-  int _pad;
-};
 #define HFB_GJK_UNKNOWN_TYPES (-99)  // status of a pair whose node types no kernel knows (reported as unsupported)
 
+// rows of the finished-pair state (by position in the class-sorted range)
+enum { FD_DIST = 0, FD_RAY = 1, FD_W = 4, FD_ROWS = FD_W + 4 * 6 };  // slot j: w0 xyz at FD_W + 6j, w1 xyz after
+enum { FI_STATUS = 0, FI_RANK, FI_ITER, FI_HINT0, FI_HINT1, FI_ROWS };
+// rows of the loop state of a running pair (by slot in the running list).  A pair that goes on into the next pass
+// has at most 3 live vertices: a rank-4 simplex either encloses the origin, which ends GJK, or is projected onto
+// one of its faces, edges or vertices.
+enum { RUN_SLOTS = 3 };
+enum { RD_RAY = 0, RD_ALPHA = 3, RD_RL = 4, RD_W = 5, RD_LW = RD_W + RUN_SLOTS * 6, RD_DIR = RD_LW + 3, RD_ROWS = RD_DIR + 3 };
+enum { RI_RANK = 0, RI_ITER, RI_HINT0, RI_HINT1, RI_VARIANT, RI_ROWS };
+
+struct Rows {  // entry `at` of row r: d[r * stride + at] / i[r * stride + at]
+  double* d;
+  int* i;
+};
+struct PassState {
+  Rows fin;              // finished pairs
+  unsigned char* done;   // per position: 1 finished in the first pass, 2 in a later pass, 0 running
+  Rows run[2];           // running pairs, two buffers, ping-ponged like the lists
+  size_t stride;         // positions of the range (rows of every buffer have this length)
+};
+
 struct PassArgs {
-  GjkSaved* state;           // one per position of the class-sorted GJK range
+  PassState st;
   const uint32_t* in_list;   // positions still running (null: the whole range)
   const unsigned* in_count;
   uint32_t* out_list;        // positions still running after this pass (null: last pass)
   unsigned* out_count;
+  Rows rin, rout;            // loop state of the pairs of in_list / out_list (entries of st.run)
   int steps;
   int which;  // k_gjk_end: the pairs with this `done` value
-  unsigned char* flags;  // k_gjk_first: 1 per position still running, for the ordered compaction (null: append by atomics)
 };
 
-__device__ __forceinline__ void append_running(const PassArgs& p, bool more, unsigned pos) {
+__device__ __forceinline__ void st3r(double* d, size_t stride, int row, unsigned at, v3 v) {
+  d[row * stride + at] = v.x;
+  d[(row + 1) * stride + at] = v.y;
+  d[(row + 2) * stride + at] = v.z;
+}
+__device__ __forceinline__ v3 ld3r(const double* d, size_t stride, int row, unsigned at) {
+  return mk(d[row * stride + at], d[(row + 1) * stride + at], d[(row + 2) * stride + at]);
+}
+
+// what pair_gjk_end and push_epa_item read of a finished pair
+__device__ __forceinline__ void save_finished(const PassState& st, unsigned pos, const GjkState& g) {
+  const size_t m = st.stride;
+  int* fi = st.fin.i;
+  double* fd = st.fin.d;
+  fi[FI_STATUS * m + pos] = g.status;
+  fi[FI_RANK * m + pos] = g.rank;
+  fi[FI_ITER * m + pos] = (int)g.iterations;
+  fi[FI_HINT0 * m + pos] = g.hint0;
+  fi[FI_HINT1 * m + pos] = g.hint1;
+  fd[FD_DIST * m + pos] = g.distance;
+  st3r(fd, m, FD_RAY, pos, g.ray);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (j < g.rank) {
+      const SV v = pick(g, j);
+      st3r(fd, m, FD_W + 6 * j, pos, v.w0);
+      st3r(fd, m, FD_W + 6 * j + 3, pos, v.w1);
+    }
+  }
+}
+// the slots at and above `rank` are not stored; they are zero here (nothing reads them: the witness points use the
+// live ones, and EPA writes a slot before it raises the rank over it)
+__device__ __forceinline__ void load_finished(const PassState& st, unsigned pos, int status, GjkState& g) {
+  const size_t m = st.stride;
+  const int* fi = st.fin.i;
+  const double* fd = st.fin.d;
+  g.status = status;
+  g.rank = fi[FI_RANK * m + pos];
+  g.iterations = (unsigned)fi[FI_ITER * m + pos];
+  g.hint0 = fi[FI_HINT0 * m + pos];
+  g.hint1 = fi[FI_HINT1 * m + pos];
+  g.distance = fd[FD_DIST * m + pos];
+  g.ray = ld3r(fd, m, FD_RAY, pos);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    SV v;
+    v.w0 = v.w1 = v.w = mk(0, 0, 0);
+    if (j < g.rank) {
+      v.w0 = ld3r(fd, m, FD_W + 6 * j, pos);
+      v.w1 = ld3r(fd, m, FD_W + 6 * j + 3, pos);
+      v.w = v.w0 - v.w1;
+    }
+    put(g, j, v);
+  }
+}
+
+// the loop state of a pair that goes on into the next pass.  L.w and L.dir are only carried from one iteration to
+// the next by the Polyak and Nesterov variants (gjk_step overwrites both before it reads them otherwise).
+__device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q, const GjkState& g, const GjkLoop& L,
+                                             bool momentum) {
+  r.i[RI_RANK * m + q] = g.rank;
+  r.i[RI_ITER * m + q] = (int)g.iterations;
+  r.i[RI_HINT0 * m + q] = g.hint0;
+  r.i[RI_HINT1 * m + q] = g.hint1;
+  st3r(r.d, m, RD_RAY, q, g.ray);
+  r.d[RD_ALPHA * m + q] = L.alpha;
+  r.d[RD_RL * m + q] = L.rl;
+#pragma unroll
+  for (int j = 0; j < RUN_SLOTS; ++j) {
+    if (j < g.rank) {
+      const SV v = pick(g, j);
+      st3r(r.d, m, RD_W + 6 * j, q, v.w0);
+      st3r(r.d, m, RD_W + 6 * j + 3, q, v.w1);
+    }
+  }
+  if (momentum) {
+    r.i[RI_VARIANT * m + q] = L.variant;
+    st3r(r.d, m, RD_LW, q, L.w);
+    st3r(r.d, m, RD_DIR, q, L.dir);
+  }
+}
+// the inverse of save_running; status and distance are those of gjk_begin (a running pair has no result yet), ssr
+// and upper_bound are recomputed as gjk_begin computes them, and the slots at and above `rank` are left unset (the
+// next support point is written there before anything reads the slot)
+__device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q, const MinkD& md, const GjkParams& P,
+                                             GjkState& g, GjkLoop& L) {
+  g.status = HFB_GJK_NO_COLLISION;
+  g.distance = 0.0;
+  g.rank = r.i[RI_RANK * m + q];
+  g.iterations = (unsigned)r.i[RI_ITER * m + q];
+  g.hint0 = r.i[RI_HINT0 * m + q];
+  g.hint1 = r.i[RI_HINT1 * m + q];
+  g.ray = ld3r(r.d, m, RD_RAY, q);
+  L.alpha = r.d[RD_ALPHA * m + q];
+  L.rl = r.d[RD_RL * m + q];
+  L.ssr = md.ssr0 + md.ssr1;
+  L.upper_bound = P.distance_upper_bound + L.ssr;
+#pragma unroll
+  for (int j = 0; j < RUN_SLOTS; ++j) {
+    if (j < g.rank) {
+      SV v;
+      v.w0 = ld3r(r.d, m, RD_W + 6 * j, q);
+      v.w1 = ld3r(r.d, m, RD_W + 6 * j + 3, q);
+      v.w = v.w0 - v.w1;
+      put(g, j, v);
+    }
+  }
+  if (P.variant != HFB_GJK_DEFAULT) {
+    L.variant = r.i[RI_VARIANT * m + q];
+    L.w = ld3r(r.d, m, RD_LW, q);
+    L.dir = ld3r(r.d, m, RD_DIR, q);
+  } else {
+    L.variant = HFB_GJK_DEFAULT;
+    L.w = L.dir = g.ray;
+  }
+}
+
+// appends `pos` to the running list if `more`; returns its slot there
+__device__ __forceinline__ unsigned append_running(const PassArgs& p, bool more, unsigned pos) {
   const unsigned m = __ballot_sync(0xffffffffu, more);
-  if (!m) return;
+  if (!m) return 0;
   const unsigned lane = threadIdx.x & 31u;
   unsigned base = 0;
   if (lane == (unsigned)(__ffs(m) - 1)) base = atomicAdd(p.out_count, (unsigned)__popc(m));
   base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
-  if (more) p.out_list[base + (unsigned)__popc(m & ((1u << lane) - 1u))] = pos;
+  const unsigned q = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+  if (more) p.out_list[q] = pos;
+  return q;
 }
 
 __global__ void __launch_bounds__(128) k_gjk_first(const BatchArgs a, const PassArgs p) {
   const unsigned lo = *a.range_lo, hi = *a.range_hi;
   const unsigned stride = gridDim.x * blockDim.x;
+  const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned k0 = lo + blockIdx.x * blockDim.x; k0 < hi; k0 += stride) {  // (warp-uniform trip count)
     const unsigned k = k0 + threadIdx.x;
     bool more = false;
+    GjkState g;
+    GjkLoop L;
     if (k < hi) {
       const unsigned i = a.index_list[k];
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
-      GjkSaved sv;
-      sv._pad = 0;
       if (!type_known(in.s1.type) || !type_known(in.s2.type)) {
-        sv.g.status = HFB_GJK_UNKNOWN_TYPES;
+        p.st.fin.i[FI_STATUS * p.st.stride + (k - lo)] = HFB_GJK_UNKNOWN_TYPES;
       } else {
         GjkSetup S;
         PairOut o;
-        pair_gjk_begin<CAP_PRIM>(in, a.P, S, sv.L, sv.g, o);
+        pair_gjk_begin<CAP_PRIM>(in, a.P, S, L, g, o);
         more = true;
-        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, sv.g, sv.L);
+        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L);
+        if (!more) save_finished(p.st, k - lo, g);
       }
-      sv.done = more ? 0 : 1;
-      p.state[k - lo] = sv;
-      if (p.flags) p.flags[k - lo] = more ? 1 : 0;
+      p.st.done[k - lo] = more ? 0 : 1;
     }
-    if (p.out_list && !p.flags) append_running(p, more, k - lo);
+    if (p.out_list) {
+      const unsigned q = append_running(p, more, k - lo);
+      if (more) save_running(p.rout, p.st.stride, q, g, L, momentum);
+    }
   }
 }
 
@@ -81,23 +221,31 @@ __global__ void __launch_bounds__(128) k_gjk_more(const BatchArgs a, const PassA
   const unsigned lo = *a.range_lo;
   const unsigned n = *p.in_count;
   const unsigned stride = gridDim.x * blockDim.x;
+  const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned q0 = blockIdx.x * blockDim.x; q0 < n; q0 += stride) {
     const unsigned q = q0 + threadIdx.x;
     bool more = false;
     unsigned pos = 0;
+    GjkState g;
+    GjkLoop L;
     if (q < n) {
       pos = p.in_list[q];
       const unsigned i = a.index_list[lo + pos];
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       GjkSetup S;
       make_setup<CAP_PRIM>(in, S);
-      GjkSaved sv = p.state[pos];
+      load_running(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L);
       more = true;
-      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, sv.g, sv.L);
-      sv.done = more ? 0 : 2;
-      p.state[pos] = sv;
+      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L);
+      if (!more) {
+        save_finished(p.st, pos, g);
+        p.st.done[pos] = 2;
+      }
     }
-    if (p.out_list) append_running(p, more, pos);
+    if (p.out_list) {
+      const unsigned qo = append_running(p, more, pos);
+      if (more) save_running(p.rout, p.st.stride, qo, g, L, momentum);
+    }
   }
 }
 
@@ -105,37 +253,68 @@ template <int MODE>
 __global__ void __launch_bounds__(128) k_gjk_end(const BatchArgs a, const PassArgs p) {
   const unsigned lo = *a.range_lo, hi = *a.range_hi;
   for (unsigned k = lo + blockIdx.x * blockDim.x + threadIdx.x; k < hi; k += gridDim.x * blockDim.x) {
-    if (p.which >= 0 && p.state[k - lo].done != p.which) continue;  // (which < 0: every pair, one launch after the last pass)
+    const unsigned pos = k - lo;
+    if (p.which >= 0 && p.st.done[pos] != p.which) continue;  // (which < 0: every pair, one launch after the last pass)
     const unsigned i = a.index_list[k];
-    const PairIn in = load_pair_in<CAP_PRIM>(a, i);
-    GjkState g = p.state[k - lo].g;
-    PairOut o;
-    if (g.status == HFB_GJK_UNKNOWN_TYPES) {
-      pair_phase1<1, CAP_PRIM, PATH_GJKROUTE>(in, a.P, o, g);  // returns at once: HFB_PATH_UNSUPPORTED
-      store_result<MODE>(a, i, o);
-      continue;
+    const int status = p.st.fin.i[FI_STATUS * p.st.stride + pos];
+    GjkState g;
+    if (status != HFB_GJK_UNKNOWN_TYPES) {
+      load_finished(p.st, pos, status, g);
+      if (status == HFB_GJK_COLLISION && a.P.compute_penetration) {  // the EPA case of pair_gjk_end
+        push_epa_item(a, i, g);
+        continue;
+      }
     }
-    // what pair_gjk_begin leaves in `o` for the extractors
-    o.cached_guess = (a.P.initial_guess == HFB_GUESS_CACHED) ? in.cached_guess : mk(1, 0, 0);
-    o.hint0 = in.hint0;
-    o.hint1 = in.hint1;
+    // what load_pair_in and pair_gjk_begin leave in `o` for the extractors
+    PairOut o;
+    o.cached_guess = mk(1, 0, 0);
+    o.hint0 = o.hint1 = 0;
     o.iterations = 0;
-    GjkSetup S;
-    make_setup<CAP_PRIM>(in, S);
-    if (pair_gjk_end(a.P, S, g, o)) push_epa_item(a, i, g);
-    else store_result<MODE>(a, i, o);
+    if (a.P.initial_guess == HFB_GUESS_CACHED) {
+      if (a.guess_in) o.cached_guess = mk(a.guess_in[3 * i], a.guess_in[3 * i + 1], a.guess_in[3 * i + 2]);
+      if (a.hint_in) {
+        o.hint0 = a.hint_in[2 * i];
+        o.hint1 = a.hint_in[2 * i + 1];
+      }
+    }
+    if (status == HFB_GJK_UNKNOWN_TYPES) {
+      set_unsupported(o);
+    } else {
+      // of what make_setup<CAP_PRIM> builds, the extractors read the first pose, `swapped` and the two radii
+      GjkSetup S;
+      S.tfa = load_xf(a.tf1[i].R);
+      S.swapped = false;
+      mink_radii(load_shape<CAP_PRIM>(a.A, a.h1[i]), load_shape<CAP_PRIM>(a.A, a.h2[i]), S.md);
+      pair_gjk_end<true>(a.P, S, g, o);
+    }
+    store_result<MODE>(a, i, o);
   }
+}
+
+// the buffers of the pass state, carved from `base` (null: only the size is wanted); returns the bytes used
+size_t carve(void* base, size_t n, PassState& st) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    void* q = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(base) + off);
+    off += (bytes + 255) & ~(size_t)255;
+    return q;
+  };
+  st.stride = n;
+  st.fin.d = static_cast<double*>(take(FD_ROWS * n * sizeof(double)));
+  st.fin.i = static_cast<int*>(take(FI_ROWS * n * sizeof(int)));
+  st.done = static_cast<unsigned char*>(take(n));
+  for (Rows& r : st.run) {
+    r.d = static_cast<double*>(take(RD_ROWS * n * sizeof(double)));
+    r.i = static_cast<int*>(take(RI_ROWS * n * sizeof(int)));
+  }
+  return off;
 }
 
 }  // namespace
 
-size_t gjk_pass_state_bytes(size_t n) { return n * sizeof(GjkSaved); }
-// flags (n bytes, rounded) + the temporary storage of the ordered compaction
-size_t gjk_pass_select_bytes(size_t n) {
-  size_t tmp = 0;
-  cub::DeviceSelect::Flagged(nullptr, tmp, cub::CountingInputIterator<uint32_t>(0), (const unsigned char*)nullptr, (uint32_t*)nullptr,
-                             (unsigned*)nullptr, (int)n);
-  return ((n + 255) & ~(size_t)255) + tmp + 256;
+size_t gjk_pass_state_bytes(size_t n) {
+  PassState st;
+  return carve(nullptr, n, st);
 }
 
 static unsigned pass_blocks(unsigned n, int num_sms) {
@@ -153,34 +332,21 @@ static void launch_end(const BatchArgs& a, int mode, PassArgs p, int which, unsi
 // first pass + extraction of the pairs it finished (their EPA items are in the queue when this returns, so that the
 // caller can start EPA on a side stream next to the remaining passes)
 int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, unsigned* counts,
-                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches, void* select_ws,
-                     bool extract_now) {
+                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches, bool extract_now) {
   if (npass < 1) return (int)cudaErrorInvalidValue;
   cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)npass * sizeof(unsigned), s);
   if (e != cudaSuccess) return (int)e;
-  // the survivors of the first pass in CLASS ORDER (a stable compaction of the class-sorted range) rather than in the
-  // order the warps happen to finish: the second pass then meets one pair class per warp, as the first did
-  unsigned char* flags = (select_ws && npass > 1) ? static_cast<unsigned char*>(select_ws) : nullptr;
-  const size_t flag_bytes = ((size_t)n + 255) & ~(size_t)255;
-  if (flags && (e = cudaMemsetAsync(flags, 0, flag_bytes, s)) != cudaSuccess) return (int)e;
   const unsigned blocks = pass_blocks(n, num_sms);
   PassArgs p;
-  p.state = static_cast<GjkSaved*>(state);
+  carve(state, n, p.st);
   p.in_list = nullptr;
   p.in_count = nullptr;
   p.out_list = npass > 1 ? list_a : nullptr;
   p.out_count = counts;
+  p.rout = p.st.run[0];
   p.steps = npass > 1 ? steps[0] : 0x7fffffff;
   p.which = 0;
-  p.flags = flags;
   k_gjk_first<<<blocks, 128, 0, s>>>(a, p);
-  if (flags) {
-    size_t tmp = gjk_pass_select_bytes(n) - flag_bytes - 256;
-    if ((e = cub::DeviceSelect::Flagged(flags + flag_bytes, tmp, cub::CountingInputIterator<uint32_t>(0), flags, list_a, counts, (int)n,
-                                        s)) != cudaSuccess)
-      return (int)e;
-    *launches += 2;  // (the select is two kernels)
-  }
   // the pairs this pass finished are extracted now only when somebody waits for their EPA items (EPA on a side
   // stream next to the remaining passes); otherwise one extraction launch after the last pass takes every pair, with
   // full warps
@@ -199,14 +365,16 @@ int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint3
   if (npass < 2) return 0;
   const unsigned blocks = pass_blocks(n, num_sms);
   PassArgs p;
-  p.state = static_cast<GjkSaved*>(state);
+  carve(state, n, p.st);
   p.which = 0;
-  p.flags = nullptr;
   for (int k = 1; k < npass; ++k) {
     const bool last = k + 1 == npass;
+    // list_a goes with run[0], list_b with run[1]
     p.in_list = (k & 1) ? list_a : list_b;
+    p.rin = p.st.run[(k & 1) ? 0 : 1];
     p.in_count = counts + (k - 1);
     p.out_list = last ? nullptr : ((k & 1) ? list_b : list_a);
+    p.rout = p.st.run[(k & 1) ? 1 : 0];
     p.out_count = counts + k;
     p.steps = last ? 0x7fffffff : steps[k];
     // the number of running pairs is only known on the device: the grid is sized for the typical survival rate of

@@ -790,7 +790,6 @@ struct Slot {
   DevBuf h1, h2, tf1, tf2, out, gin, hin, gout, hout, queue, counters, lists, retry, bvh_ws, bvh_cnt, extra, ccnt, okeys, ohist, olist;
   DevBuf qprep, qstacks, qtl, qws, qsv;  // task-system mesh-shape walk (hfb_bvhq.cu)
   DevBuf hsort;                      // hfb_hullsort.cu scratch
-  DevBuf gsel;                       // GJK passes: flags + scratch of the ordered compaction
   DevBuf gstate, glist, gcnt;        // GJK passes (hfb_gjkpass.cu): solver state, two lists of running pairs, counts
   DevBuf pi, pj, cmp;                // object-table batches: pair indices of the chunk; compact results
 };
@@ -843,7 +842,6 @@ struct hfb_ctx {
   int bvh_gens = 2;    // HFB_BVH_GENS: generations of BV items per cycle of k_bvhq
   int bvh_spec_big = 300;  // HFB_BVH_SPEC_BIG: items more before subtrees of up to 128 triangles are speculated
   int hull_sort = 1;      // HFB_HULL_SORT: second sort key (first operand's handle) inside the hull / triangle class
-  int gjk_ordered = 0;    // HFB_GJK_ORDERED=1: the second GJK pass takes the survivors of the first in class order (off by default)
   int epa_resume = 8192;  // HFB_EPA_RESUME: retries per batch that continue from the state tier 0 reached (5 KB each)
   int bvh_chunk = 6;   // HFB_BVH_GJK_CHUNK: GJK iterations a leaf item runs before it parks its state
   int bvh_spec = 200;  // HFB_BVH_SPEC: items a query uses before it may speculate on subtrees (< 0: never)
@@ -1138,14 +1136,13 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
           CK(sl.gstate.reserve(gjk_pass_state_bytes(n)));
           CK(sl.glist.reserve(2 * (size_t)n * sizeof(uint32_t)));
           CK(sl.gcnt.reserve(8 * sizeof(unsigned)));
-          if (ctx->gjk_ordered) CK(sl.gsel.reserve(gjk_pass_select_bytes(n)));
           int nl = 0;
           uint32_t* la = static_cast<uint32_t*>(sl.glist.p);
           const bool early_epa = ctx->gjk_npass > 1 && ctx->epa_overlap && want_epa;
           {
             KTimer kt(ctx, ws, 0);
             if (gjk_passes_first(ag, MODE, n, sl.gstate.p, la, static_cast<unsigned*>(sl.gcnt.p), ctx->gjk_steps, ctx->gjk_npass,
-                                 ctx->num_sms, ws, &nl, ctx->gjk_ordered ? sl.gsel.p : nullptr, early_epa) != 0)
+                                 ctx->num_sms, ws, &nl, early_epa) != 0)
               return fail(ctx, HFB_ERR_CUDA, "GJK pass launch failed");
           }
           // EPA of the pairs the first pass finished starts on the side stream, next to the remaining passes (which
@@ -1832,7 +1829,6 @@ int hfb_ctx_create(int device, hfb_ctx** out) {
   if (const char* bc = getenv("HFB_BVH_GJK_CHUNK")) c->bvh_chunk = atoi(bc) > 0 ? atoi(bc) : 1;
   if (const char* hs = getenv("HFB_HULL_SORT")) c->hull_sort = atoi(hs) != 0;
   if (const char* hp = getenv("HFB_HOST_PIPE")) c->host_pipe = atoi(hp) < 0 ? 0 : atoi(hp);
-  if (const char* go = getenv("HFB_GJK_ORDERED")) c->gjk_ordered = atoi(go) != 0;
   if (const char* er = getenv("HFB_EPA_RESUME")) c->epa_resume = atoi(er) > 0 ? atoi(er) : 0;
   if (const char* gp = getenv("HFB_GJK_PASSES")) {
     c->gjk_npass = 0;
@@ -1874,7 +1870,7 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   cudaDeviceSynchronize();
   hfb_comm_destroy(c);
   auto rel = [](Slot& s) {
-    DevBuf* bs[] = {&s.h1, &s.h2, &s.tf1, &s.tf2, &s.out, &s.gin, &s.hin, &s.gout, &s.hout, &s.queue, &s.counters, &s.lists, &s.retry, &s.bvh_ws, &s.bvh_cnt, &s.extra, &s.ccnt, &s.okeys, &s.ohist, &s.olist, &s.qprep, &s.qstacks, &s.qtl, &s.qws, &s.qsv, &s.gstate, &s.glist, &s.gcnt, &s.pi, &s.pj, &s.cmp, &s.cont, &s.gsel, &s.hsort};
+    DevBuf* bs[] = {&s.h1, &s.h2, &s.tf1, &s.tf2, &s.out, &s.gin, &s.hin, &s.gout, &s.hout, &s.queue, &s.counters, &s.lists, &s.retry, &s.bvh_ws, &s.bvh_cnt, &s.extra, &s.ccnt, &s.okeys, &s.ohist, &s.olist, &s.qprep, &s.qstacks, &s.qtl, &s.qws, &s.qsv, &s.gstate, &s.glist, &s.gcnt, &s.pi, &s.pj, &s.cmp, &s.cont, &s.hsort};
     for (DevBuf* b : bs) b->release();
     if (s.stream) cudaStreamDestroy(s.stream);
     if (s.epa_stream) cudaStreamDestroy(s.epa_stream);

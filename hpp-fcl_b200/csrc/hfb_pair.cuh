@@ -108,6 +108,13 @@ HFB_HD unsigned pack_status(int gjk, int epa, int path) {
   return ((unsigned)gjk & 0xffu) | (((unsigned)epa & 0xffu) << 8) | (((unsigned)path & 0xffu) << 16);
 }
 
+// the record of a pair no kernel can compute (the cached guess, hints and iterations are left as they are)
+HFB_HD void set_unsupported(PairOut& o) {
+  o.distance = DBL_MAX;
+  o.p1 = o.p2 = o.normal = nan3();
+  o.status = pack_status(0, 0, HFB_PATH_UNSUPPORTED);
+}
+
 // world-frame re-centring shared by the GJK and EPA extractors
 // (narrowphase.h:632-635, 707-710)
 HFB_HD void recentre(const xf& tfa, double distance, v3& p1, v3& p2, v3& normal) {
@@ -142,7 +149,8 @@ HFB_HD void pair_gjk_begin(const PairIn& in, const SolverP& P, GjkSetup& S, GjkL
   const v3 guess = initial_guess(P, in, S);
   gjk_begin(S.md, P.gjk, guess, in.hint0, in.hint1, g, L);
 }
-// returns true when EPA must still run (g holds GJK's final simplex)
+// returns true when EPA must still run (g holds GJK's final simplex); INL: see gjk_witness
+template <bool INL = false>
 HFB_HD bool pair_gjk_end(const SolverP& P, const GjkSetup& S, GjkState& g, PairOut& o) {
   o.iterations = g.iterations & 0xffffu;
   o.status = pack_status(g.status, HFB_EPA_DID_NOT_RUN, HFB_PATH_GJK);
@@ -154,7 +162,7 @@ HFB_HD bool pair_gjk_end(const SolverP& P, const GjkSetup& S, GjkState& g, PairO
       o.hint0 = g.hint0;
       o.hint1 = g.hint1;
       o.distance = g.distance;
-      gjk_witness(g, S.md, o.p1, o.p2, o.normal);
+      gjk_witness<INL>(g, S.md, o.p1, o.p2, o.normal);
       recentre(S.tfa, o.distance, o.p1, o.p2, o.normal);
       unswap(S, o);
     } break;
@@ -188,9 +196,7 @@ HFB_HD bool pair_phase1(const PairIn& in, const SolverP& P, PairOut& o, GjkState
   o.hint1 = in.hint1;
   o.iterations = 0;
   if (!type_known(t1) || !type_known(t2)) {
-    o.distance = DBL_MAX;
-    o.p1 = o.p2 = o.normal = nan3();
-    o.status = pack_status(0, 0, HFB_PATH_UNSUPPORTED);
+    set_unsupported(o);
     return false;
   }
   if (is_plane_type(t1) || is_plane_type(t2)) {
@@ -204,9 +210,7 @@ HFB_HD bool pair_phase1(const PairIn& in, const SolverP& P, PairOut& o, GjkState
       o.normal = w.n;
       o.status = pack_status(HFB_GJK_DID_NOT_RUN, HFB_EPA_DID_NOT_RUN, HFB_PATH_CLOSED_FORM);
     } else {
-      o.distance = DBL_MAX;
-      o.p1 = o.p2 = o.normal = nan3();
-      o.status = pack_status(0, 0, HFB_PATH_UNSUPPORTED);
+      set_unsupported(o);
     }
     return false;
   }
@@ -233,9 +237,7 @@ HFB_HD bool pair_phase1(const PairIn& in, const SolverP& P, PairOut& o, GjkState
   }
 
   if (!(PATHS & PATH_GJKROUTE)) {  // mis-binned pair: cannot happen (k_bin_* and is_closed_form agree)
-    o.distance = DBL_MAX;
-    o.p1 = o.p2 = o.normal = nan3();
-    o.status = pack_status(0, 0, HFB_PATH_UNSUPPORTED);
+    set_unsupported(o);
     return false;
   }
   if ((CAPS & CAP_TRI) && t1 == HFB_GEOM_TRIANGLE && t2 == HFB_GEOM_TRIANGLE) {
