@@ -42,6 +42,8 @@
 // at 1); HFB_GC / HFB_GE override them per context.
 #define HFB_GC_DEFAULT 2
 #define HFB_GE_DEFAULT 8
+// lanes per pair of the EPA kernel's second tier (k_epa<G,CAPS,MODE,1>), whatever HFB_GE asks for the first
+#define HFB_GE_TIER1 32
 
 // pair classes of the device-side counting sort (k_bin_*): bins [0,9) closed-form
 // combos (bin 8: a plane or halfspace against a primitive or another plane), [9,45) GJK-routed
@@ -301,6 +303,9 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
     k = __shfl_sync(Coop<G>::mask(), k, (threadIdx.x & 31u) & ~(unsigned)(G - 1));
     if (k >= hi) break;
     const unsigned k_pos = k;  // (tier 1: position in the retry list = slot of the continuation record)
+    // tier 0 hands the queue out from its end: k_gjk_end fills it in pair-class order, with the cylinder classes last.
+    // Their runs are the longest, so starting them first shortens the end of the launch
+    if (TIER == 0) k = lo + hi - 1 - k;
     if (TIER == 1) k = a.retry[k];
     const EpaItem* it = a.queue + k;
     const unsigned i = it->pair;
@@ -954,11 +959,17 @@ int launch_epa(hfb_ctx* ctx, const BatchArgs& a, cudaStream_t s) {
 
 template <int CAPS, int MODE, int TIER>
 int launch_epa_g(hfb_ctx* ctx, const BatchArgs& a, cudaStream_t s) {
-  switch (ctx->ge) {
-    case 4: return launch_epa<4, CAPS, MODE, TIER>(ctx, a, s);
-    case 8: return launch_epa<8, CAPS, MODE, TIER>(ctx, a, s);
-    case 16: return launch_epa<16, CAPS, MODE, TIER>(ctx, a, s);
-    default: return launch_epa<32, CAPS, MODE, TIER>(ctx, a, s);
+  // tier 1 runs the few pairs that outgrew tier 0 on an almost idle GPU: its time is the serial chain of the longest of
+  // them, which wide groups shorten (the closest-face scan and the new faces' geometry are spread over the lanes)
+  if constexpr (TIER == 1) {
+    return launch_epa<HFB_GE_TIER1, CAPS, MODE, 1>(ctx, a, s);
+  } else {
+    switch (ctx->ge) {
+      case 4: return launch_epa<4, CAPS, MODE, 0>(ctx, a, s);
+      case 8: return launch_epa<8, CAPS, MODE, 0>(ctx, a, s);
+      case 16: return launch_epa<16, CAPS, MODE, 0>(ctx, a, s);
+      default: return launch_epa<32, CAPS, MODE, 0>(ctx, a, s);
+    }
   }
 }
 template <int MODE>
