@@ -20,6 +20,12 @@ namespace hfb {
 struct SV {  // GJK::SimplexV (gjk.h:55-61)
   v3 w0, w1, w;
 };
+// A vertex whose support points w0 / w1 are kept in slot `slot` of a per-thread store outside the registers (the GJK
+// passes, hfb_gjkpass.cu): the iterations only read w.
+struct SVSlot {
+  v3 w;
+  int slot;
+};
 
 struct GjkParams {  // per-batch constants (GJKSolver::set, narrowphase.h:162-244)
   double tolerance;
@@ -30,8 +36,9 @@ struct GjkParams {  // per-batch constants (GJKSolver::set, narrowphase.h:162-24
   int criterion_type;
 };
 
-struct GjkState {
-  SV s0, s1, s2, s3;  // simplex.vertex[0..3]
+template <class V>
+struct GjkStateT {
+  V s0, s1, s2, s3;  // simplex.vertex[0..3]
   int rank;
   v3 ray;
   double distance;
@@ -39,9 +46,12 @@ struct GjkState {
   int hint0, hint1;
   unsigned iterations;
 };
+using GjkState = GjkStateT<SV>;
 
-HFB_HD SV pick(const GjkState& g, int i) { return i == 0 ? g.s0 : (i == 1 ? g.s1 : (i == 2 ? g.s2 : g.s3)); }
-HFB_HD void put(GjkState& g, int i, const SV& v) {
+template <class V>
+HFB_HD V pick(const GjkStateT<V>& g, int i) { return i == 0 ? g.s0 : (i == 1 ? g.s1 : (i == 2 ? g.s2 : g.s3)); }
+template <class V>
+HFB_HD void put(GjkStateT<V>& g, int i, const V& v) {
   if (i == 0) g.s0 = v;
   else if (i == 1) g.s1 = v;
   else if (i == 2) g.s2 = v;
@@ -57,6 +67,17 @@ HFB_HD SV gjk_support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, i
   return sv;
 }
 
+// Where gjk_step appends a support point: InRegs keeps the whole SV in the simplex (every caller but the GJK passes,
+// which keep w0 / w1 in a per-thread store of their own, SlotStore in hfb_gjkpass.cu).  append puts `nv` at
+// simplex.vertex[g.rank] and returns its w.
+struct InRegs {
+  using V = SV;
+  HFB_HD v3 append(GjkState& g, const SV& nv) const {
+    put(g, g.rank, nv);
+    return nv.w;
+  }
+};
+
 // region codes of the simplex projections
 enum { RG_A = 0, RG_AB, RG_AC, RG_AD, RG_ABC, RG_ACD, RG_ADB, RG_INSIDE };
 
@@ -68,8 +89,10 @@ HFB_HD v3 ray_segment(v3 A, v3 X, v3 AX, double t) {
 // originToTriangle (:517-541), ABCdotAO != 0
 HFB_HD v3 ray_triangle(v3 N, double NdotAO) { return (-NdotAO / sqn(N)) * N; }
 
+// The projections read only w of each vertex and move whole vertices (V: SV or SVSlot).
 // projectLineOrigin (:543-569). A = newest = s1, B = s0.
-HFB_HD bool project_line(GjkState& g) {
+template <class V>
+HFB_HD bool project_line(GjkStateT<V>& g) {
   const v3 A = g.s1.w, B = g.s0.w;
   const v3 AB = B - A;
   const double d = dot(AB, -A);
@@ -89,7 +112,8 @@ HFB_HD bool project_line(GjkState& g) {
 }
 
 // projectTriangleOrigin (:571-611). A = s2, B = s1, C = s0.
-HFB_HD bool project_triangle(GjkState& g) {
+template <class V>
+HFB_HD bool project_triangle(GjkStateT<V>& g) {
   const v3 A = g.s2.w, B = g.s1.w, C = g.s0.w;
   const v3 AB = B - A, AC = C - A, ABC = cross(AB, AC);
   int region;
@@ -139,7 +163,7 @@ HFB_HD bool project_triangle(GjkState& g) {
         return true;
       }
       if (!(dAO > 0)) {  // next = [b, c, a]
-        SV tmp = g.s0;
+        V tmp = g.s0;
         g.s0 = g.s1;
         g.s1 = tmp;
       }
@@ -150,7 +174,8 @@ HFB_HD bool project_triangle(GjkState& g) {
 }
 
 // projectTetrahedraOrigin (:613-1010). A = s3, B = s2, C = s1, D = s0.
-HFB_HD bool project_tetra(GjkState& g) {
+template <class V>
+HFB_HD bool project_tetra(GjkStateT<V>& g) {
   const v3 A = g.s3.w, B = g.s2.w, C = g.s1.w, D = g.s0.w;
   const double aa = sqn(A);
   const double da = dot(D, A), db = dot(D, B), dc = dot(D, C), dd = dot(D, D);
@@ -229,7 +254,7 @@ HFB_HD bool project_tetra(GjkState& g) {
     const v3 X = isB ? B : (isC ? C : D);
     const double t = isB ? -ba_aa : (isC ? -ca_aa : -da_aa);
     g.ray = ray_segment(A, X, X - A, t);
-    const SV sx = isB ? g.s2 : (isC ? g.s1 : g.s0);
+    const V sx = isB ? g.s2 : (isC ? g.s1 : g.s0);
     g.s0 = sx;
     g.s1 = g.s3;
     g.rank = 2;
@@ -240,8 +265,8 @@ HFB_HD bool project_tetra(GjkState& g) {
   const bool tABC = region == RG_ABC, tACD = region == RG_ACD;
   const v3 X = tABC ? B : (tACD ? C : D);
   const v3 Y = tABC ? C : (tACD ? D : B);
-  const SV sx = tABC ? g.s2 : (tACD ? g.s1 : g.s0);
-  const SV sy = tABC ? g.s1 : (tACD ? g.s0 : g.s2);
+  const V sx = tABC ? g.s2 : (tACD ? g.s1 : g.s0);
+  const V sy = tABC ? g.s1 : (tACD ? g.s0 : g.s2);
   const double dAO = tABC ? -C_axb : (tACD ? -D_axc : D_axb);
   const v3 N = cross(X - A, Y - A);
   g.rank = 3;
@@ -293,7 +318,9 @@ struct GjkLoop {  // what the do-while of the reference carries from one iterati
   v3 w, dir;
 };
 
-HFB_HD void gjk_begin(const MinkD& md, const GjkParams& P, v3 guess, int hint0, int hint1, GjkState& g, GjkLoop& L) {
+template <class V>
+HFB_HD void gjk_begin(const MinkD& md, const GjkParams& P, v3 guess, int hint0, int hint1, GjkStateT<V>& g,
+                      GjkLoop& L) {
   L.alpha = 0;
   g.iterations = 0;
   L.ssr = md.ssr0 + md.ssr1;
@@ -317,10 +344,11 @@ HFB_HD void gjk_begin(const MinkD& md, const GjkParams& P, v3 guess, int hint0, 
   L.dir = g.ray;
 }
 
-// one pass through the body of the do-while; returns whether the loop goes on
-template <int G, int CAPS>
-HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const GjkParams& P, GjkState& g,
-                     GjkLoop& L) {
+// one pass through the body of the do-while; returns whether the loop goes on.  `st` appends the new support point
+// (InRegs, or the passes' SlotStore; its vertex type is the simplex's).
+template <int G, int CAPS, class Store = InRegs>
+HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const GjkParams& P,
+                     GjkStateT<typename Store::V>& g, GjkLoop& L, const Store& st = Store()) {
   const double tol = P.tolerance;
   // check A (:228-243)
   if (L.rl < tol) {
@@ -349,9 +377,8 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
 
   // appendVertex(curr_simplex, -dir, support_hint) (:281)
   const SV nv = gjk_support<G, CAPS>(sa, sb, md, -L.dir, g.hint0, g.hint1);
-  put(g, g.rank, nv);
+  L.w = st.append(g, nv);
   g.rank += 1;
-  L.w = nv.w;
 
   // check B (:288-293)
   const double omega = dot(L.dir, L.w) / nrm(L.dir);

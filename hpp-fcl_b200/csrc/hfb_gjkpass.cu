@@ -18,9 +18,50 @@
 // live simplex vertex (w = w0 - w1 is not stored: gjk_support computed it that way); a pair still running leaves its
 // loop state, 56 B plus 48 B per live vertex (plus 52 B for the Polyak and Nesterov variants), at its slot in the
 // list of running pairs, where the next pass reads it densely.
+//
+// Inside k_gjk_first and k_gjk_more a simplex vertex is w and a slot id (SVSlot): the support points w0 / w1, which
+// the iterations never read, wait in a per-thread store in shared memory (SlotStore) until the pair's state is saved.
+// That leaves registers for 3 blocks of 128 threads per SM instead of 2.
 #include "hfb_gjkpass.h"
 
 namespace {
+
+enum { PASS_THREADS = 128, PASS_BLOCKS_PER_SM = 3 };  // k_gjk_first / k_gjk_more: block size, resident blocks per SM
+
+// w0 / w1 of the simplex vertices of the passes: 4 slots per thread, laid out [slot][component][thread] so that the
+// lanes of a warp touch consecutive doubles (24 KB per block).  gjk_step appends a support point in the lowest slot no
+// live vertex uses: at most 3 vertices are live when it appends, so one is always free.
+struct SlotStore {
+  using V = SVSlot;
+  double* col;  // this thread's column: component c of slot j at col[(6 * j + c) * PASS_THREADS]
+
+  __device__ __forceinline__ void st(int j, v3 w0, v3 w1) const {
+    double* p = col + 6 * j * PASS_THREADS;
+    p[0] = w0.x;
+    p[PASS_THREADS] = w0.y;
+    p[2 * PASS_THREADS] = w0.z;
+    p[3 * PASS_THREADS] = w1.x;
+    p[4 * PASS_THREADS] = w1.y;
+    p[5 * PASS_THREADS] = w1.z;
+  }
+  __device__ __forceinline__ void ld(int j, v3& w0, v3& w1) const {
+    const double* p = col + 6 * j * PASS_THREADS;
+    w0 = mk(p[0], p[PASS_THREADS], p[2 * PASS_THREADS]);
+    w1 = mk(p[3 * PASS_THREADS], p[4 * PASS_THREADS], p[5 * PASS_THREADS]);
+  }
+  __device__ __forceinline__ v3 append(GjkStateT<SVSlot>& g, const SV& nv) const {
+    unsigned used = 0;
+    if (g.rank > 0) used |= 1u << g.s0.slot;
+    if (g.rank > 1) used |= 1u << g.s1.slot;
+    if (g.rank > 2) used |= 1u << g.s2.slot;
+    SVSlot v;
+    v.w = nv.w;
+    v.slot = __ffs(~used) - 1;
+    st(v.slot, nv.w0, nv.w1);
+    put(g, g.rank, v);
+    return nv.w;
+  }
+};
 
 #define HFB_GJK_UNKNOWN_TYPES (-99)  // status of a pair whose node types no kernel knows (reported as unsupported)
 
@@ -66,7 +107,8 @@ __device__ __forceinline__ v3 ld3r(const double* d, size_t stride, int row, unsi
 }
 
 // what pair_gjk_end and push_epa_item read of a finished pair
-__device__ __forceinline__ void save_finished(const PassState& st, unsigned pos, const GjkState& g) {
+__device__ __forceinline__ void save_finished(const PassState& st, unsigned pos, const GjkStateT<SVSlot>& g,
+                                              const SlotStore& ss) {
   const size_t m = st.stride;
   int* fi = st.fin.i;
   double* fd = st.fin.d;
@@ -80,9 +122,10 @@ __device__ __forceinline__ void save_finished(const PassState& st, unsigned pos,
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     if (j < g.rank) {
-      const SV v = pick(g, j);
-      st3r(fd, m, FD_W + 6 * j, pos, v.w0);
-      st3r(fd, m, FD_W + 6 * j + 3, pos, v.w1);
+      v3 w0, w1;
+      ss.ld(pick(g, j).slot, w0, w1);
+      st3r(fd, m, FD_W + 6 * j, pos, w0);
+      st3r(fd, m, FD_W + 6 * j + 3, pos, w1);
     }
   }
 }
@@ -114,8 +157,8 @@ __device__ __forceinline__ void load_finished(const PassState& st, unsigned pos,
 
 // the loop state of a pair that goes on into the next pass.  L.w and L.dir are only carried from one iteration to
 // the next by the Polyak and Nesterov variants (gjk_step overwrites both before it reads them otherwise).
-__device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q, const GjkState& g, const GjkLoop& L,
-                                             bool momentum) {
+__device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q, const GjkStateT<SVSlot>& g,
+                                             const GjkLoop& L, bool momentum, const SlotStore& ss) {
   r.i[RI_RANK * m + q] = g.rank;
   r.i[RI_ITER * m + q] = (int)g.iterations;
   r.i[RI_HINT0 * m + q] = g.hint0;
@@ -126,9 +169,10 @@ __device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q
 #pragma unroll
   for (int j = 0; j < RUN_SLOTS; ++j) {
     if (j < g.rank) {
-      const SV v = pick(g, j);
-      st3r(r.d, m, RD_W + 6 * j, q, v.w0);
-      st3r(r.d, m, RD_W + 6 * j + 3, q, v.w1);
+      v3 w0, w1;
+      ss.ld(pick(g, j).slot, w0, w1);
+      st3r(r.d, m, RD_W + 6 * j, q, w0);
+      st3r(r.d, m, RD_W + 6 * j + 3, q, w1);
     }
   }
   if (momentum) {
@@ -138,10 +182,10 @@ __device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q
   }
 }
 // the inverse of save_running; status and distance are those of gjk_begin (a running pair has no result yet), ssr
-// and upper_bound are recomputed as gjk_begin computes them, and the slots at and above `rank` are left unset (the
-// next support point is written there before anything reads the slot)
+// and upper_bound are recomputed as gjk_begin computes them.  Vertex j's support points go to store slot j; the
+// vertices at and above `rank` are left unset (the next support point is written there before anything reads them).
 __device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q, const MinkD& md, const GjkParams& P,
-                                             GjkState& g, GjkLoop& L) {
+                                             GjkStateT<SVSlot>& g, GjkLoop& L, const SlotStore& ss) {
   g.status = HFB_GJK_NO_COLLISION;
   g.distance = 0.0;
   g.rank = r.i[RI_RANK * m + q];
@@ -156,10 +200,12 @@ __device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q
 #pragma unroll
   for (int j = 0; j < RUN_SLOTS; ++j) {
     if (j < g.rank) {
-      SV v;
-      v.w0 = ld3r(r.d, m, RD_W + 6 * j, q);
-      v.w1 = ld3r(r.d, m, RD_W + 6 * j + 3, q);
-      v.w = v.w0 - v.w1;
+      const v3 w0 = ld3r(r.d, m, RD_W + 6 * j, q);
+      const v3 w1 = ld3r(r.d, m, RD_W + 6 * j + 3, q);
+      ss.st(j, w0, w1);
+      SVSlot v;
+      v.w = w0 - w1;
+      v.slot = j;
       put(g, j, v);
     }
   }
@@ -186,14 +232,16 @@ __device__ __forceinline__ unsigned append_running(const PassArgs& p, bool more,
   return q;
 }
 
-__global__ void __launch_bounds__(128) k_gjk_first(const BatchArgs a, const PassArgs p) {
+__global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_first(const BatchArgs a, const PassArgs p) {
+  __shared__ double store_rows[4 * 6 * PASS_THREADS];
+  const SlotStore ss{store_rows + threadIdx.x};
   const unsigned lo = *a.range_lo, hi = *a.range_hi;
   const unsigned stride = gridDim.x * blockDim.x;
   const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned k0 = lo + blockIdx.x * blockDim.x; k0 < hi; k0 += stride) {  // (warp-uniform trip count)
     const unsigned k = k0 + threadIdx.x;
     bool more = false;
-    GjkState g;
+    GjkStateT<SVSlot> g;
     GjkLoop L;
     if (k < hi) {
       const unsigned i = a.index_list[k];
@@ -205,19 +253,21 @@ __global__ void __launch_bounds__(128) k_gjk_first(const BatchArgs a, const Pass
         PairOut o;
         pair_gjk_begin<CAP_PRIM>(in, a.P, S, L, g, o);
         more = true;
-        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L);
-        if (!more) save_finished(p.st, k - lo, g);
+        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
+        if (!more) save_finished(p.st, k - lo, g, ss);
       }
       p.st.done[k - lo] = more ? 0 : 1;
     }
     if (p.out_list) {
       const unsigned q = append_running(p, more, k - lo);
-      if (more) save_running(p.rout, p.st.stride, q, g, L, momentum);
+      if (more) save_running(p.rout, p.st.stride, q, g, L, momentum, ss);
     }
   }
 }
 
-__global__ void __launch_bounds__(128) k_gjk_more(const BatchArgs a, const PassArgs p) {
+__global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_more(const BatchArgs a, const PassArgs p) {
+  __shared__ double store_rows[4 * 6 * PASS_THREADS];
+  const SlotStore ss{store_rows + threadIdx.x};
   const unsigned lo = *a.range_lo;
   const unsigned n = *p.in_count;
   const unsigned stride = gridDim.x * blockDim.x;
@@ -226,7 +276,7 @@ __global__ void __launch_bounds__(128) k_gjk_more(const BatchArgs a, const PassA
     const unsigned q = q0 + threadIdx.x;
     bool more = false;
     unsigned pos = 0;
-    GjkState g;
+    GjkStateT<SVSlot> g;
     GjkLoop L;
     if (q < n) {
       pos = p.in_list[q];
@@ -234,17 +284,17 @@ __global__ void __launch_bounds__(128) k_gjk_more(const BatchArgs a, const PassA
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       GjkSetup S;
       make_setup<CAP_PRIM>(in, S);
-      load_running(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L);
+      load_running(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L, ss);
       more = true;
-      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L);
+      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
       if (!more) {
-        save_finished(p.st, pos, g);
+        save_finished(p.st, pos, g, ss);
         p.st.done[pos] = 2;
       }
     }
     if (p.out_list) {
       const unsigned qo = append_running(p, more, pos);
-      if (more) save_running(p.rout, p.st.stride, qo, g, L, momentum);
+      if (more) save_running(p.rout, p.st.stride, qo, g, L, momentum, ss);
     }
   }
 }
@@ -317,9 +367,10 @@ size_t gjk_pass_state_bytes(size_t n) {
   return carve(nullptr, n, st);
 }
 
+// one block per PASS_THREADS pairs, at most 16 waves of resident blocks (the kernels stride over the rest)
 static unsigned pass_blocks(unsigned n, int num_sms) {
-  unsigned blocks = (n + 127) / 128;
-  const unsigned cap = (unsigned)num_sms * 32u;
+  unsigned blocks = (n + PASS_THREADS - 1) / PASS_THREADS;
+  const unsigned cap = (unsigned)num_sms * PASS_BLOCKS_PER_SM * 16u;
   if (blocks > cap) blocks = cap;
   return blocks ? blocks : 1u;
 }
@@ -346,7 +397,7 @@ int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint
   p.rout = p.st.run[0];
   p.steps = npass > 1 ? steps[0] : 0x7fffffff;
   p.which = 0;
-  k_gjk_first<<<blocks, 128, 0, s>>>(a, p);
+  k_gjk_first<<<blocks, PASS_THREADS, 0, s>>>(a, p);
   // the pairs this pass finished are extracted now only when somebody waits for their EPA items (EPA on a side
   // stream next to the remaining passes); otherwise one extraction launch after the last pass takes every pair, with
   // full warps
@@ -378,10 +429,11 @@ int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint3
     p.out_count = counts + k;
     p.steps = last ? 0x7fffffff : steps[k];
     // the number of running pairs is only known on the device: the grid is sized for the typical survival rate of
-    // a pass and strides over whatever there is
+    // a pass and strides over whatever there is, but never fills less than one wave of resident blocks
+    const unsigned wave = (unsigned)num_sms * PASS_BLOCKS_PER_SM;
     unsigned b = blocks >> (k < 3 ? k : 3);
-    if (b < (unsigned)num_sms * 2u) b = (unsigned)num_sms * 2u < blocks ? (unsigned)num_sms * 2u : blocks;
-    k_gjk_more<<<b, 128, 0, s>>>(a, p);
+    if (b < wave) b = wave < blocks ? wave : blocks;
+    k_gjk_more<<<b, PASS_THREADS, 0, s>>>(a, p);
     ++*launches;
   }
   launch_end(a, mode, p, first_extracted ? 2 : -1, blocks, s);

@@ -139,8 +139,9 @@ enum { PATH_CLOSED = 1, PATH_GJKROUTE = 2, PATH_BOTH = 3 };
 
 // the general GJK route of phase 1 in three pieces (set-up, iterations, extraction), so that the
 // primitive-pair kernel can refill lanes between iterations; pair_phase1 chains them for everybody else
-template <int CAPS>
-HFB_HD void pair_gjk_begin(const PairIn& in, const SolverP& P, GjkSetup& S, GjkLoop& L, GjkState& g, PairOut& o) {
+template <int CAPS, class V>
+HFB_HD void pair_gjk_begin(const PairIn& in, const SolverP& P, GjkSetup& S, GjkLoop& L, GjkStateT<V>& g,
+                           PairOut& o) {
   o.cached_guess = (P.initial_guess == HFB_GUESS_CACHED) ? in.cached_guess : mk(1, 0, 0);
   o.hint0 = in.hint0;
   o.hint1 = in.hint1;
