@@ -121,7 +121,8 @@ __device__ __forceinline__ void st3(double* p, v3 v) {
 }
 __device__ __forceinline__ v3 ld3(const double* p) { return mk(p[0], p[1], p[2]); }
 
-__device__ __forceinline__ void push_epa_item(const BatchArgs& a, unsigned i, const GjkState& g) {
+template <class V>
+__device__ __forceinline__ EpaItem* new_epa_item(const BatchArgs& a, unsigned i, const GjkStateT<V>& g) {
   const unsigned slot = atomicAdd(a.queue_count, 1u);
   atomicAdd(a.queue_count + 1, 1u);
   EpaItem* it = a.queue + slot;
@@ -130,6 +131,24 @@ __device__ __forceinline__ void push_epa_item(const BatchArgs& a, unsigned i, co
   it->hint0 = g.hint0;
   it->hint1 = g.hint1;
   it->gjk_iterations = g.iterations;
+  return it;
+}
+// the item of a simplex whose support points sit in a store of the caller's (the GJK passes' SlotStore); the
+// vertices at and above `rank` are written as zeros
+template <class Store>
+__device__ __forceinline__ void push_epa_item(const BatchArgs& a, unsigned i, const GjkStateT<typename Store::V>& g,
+                                              const Store& st) {
+  EpaItem* it = new_epa_item(a, i, g);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    v3 w0 = mk(0, 0, 0), w1 = mk(0, 0, 0);
+    if (j < g.rank) st.support_points(pick(g, j), w0, w1);
+    st3(it->w0 + 3 * j, w0);
+    st3(it->w1 + 3 * j, w1);
+  }
+}
+__device__ __forceinline__ void push_epa_item(const BatchArgs& a, unsigned i, const GjkState& g) {
+  EpaItem* it = new_epa_item(a, i, g);
   st3(it->w0 + 0, g.s0.w0);
   st3(it->w1 + 0, g.s0.w1);
   st3(it->w0 + 3, g.s1.w0);

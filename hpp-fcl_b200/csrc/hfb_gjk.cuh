@@ -67,14 +67,24 @@ HFB_HD SV gjk_support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, i
   return sv;
 }
 
-// Where gjk_step appends a support point: InRegs keeps the whole SV in the simplex (every caller but the GJK passes,
-// which keep w0 / w1 in a per-thread store of their own, SlotStore in hfb_gjkpass.cu).  append puts `nv` at
-// simplex.vertex[g.rank] and returns its w.
+// Where gjk_step appends a support point and the witness points read them back: InRegs keeps the whole SV in the
+// simplex (every caller but the GJK passes, which keep w0 / w1 in a per-thread store of their own, SlotStore in
+// hfb_gjkpass.cu).  append puts `nv` at simplex.vertex[g.rank] and returns its w; support_points gives a vertex's
+// w0 / w1; inline_projections: closest_points_inl inlines the triangle projection of a rank-3 simplex, and the segment
+// projections it calls, instead of calling them out of line (in a kernel held to few registers an out-of-line call
+// saves and restores registers in local memory).  The tetrahedron projection is always called out of line: GJK's
+// witness points never reach it (a rank-4 simplex encloses the origin, which is a collision), and inlined it would
+// add ~20 KB of code.
 struct InRegs {
   using V = SV;
+  static constexpr bool inline_projections = false;
   HFB_HD v3 append(GjkState& g, const SV& nv) const {
     put(g, g.rank, nv);
     return nv.w;
+  }
+  HFB_HD void support_points(const SV& v, v3& w0, v3& w1) const {
+    w0 = v.w0;
+    w1 = v.w1;
   }
 };
 
@@ -455,7 +465,9 @@ HFB_HD void pset(Param4& r, int i, double v) {
   else if (i == 2) r.p2 = v;
   else r.p3 = v;
 }
-HFB_HD_NOINLINE Param4 proj_line_origin(v3 a, v3 b) {
+// The segment and triangle projections are called out of line (one copy per kernel) or, in their _inl form with INL
+// set, inlined together with the projections they call (see InRegs::inline_projections).
+HFB_HD Param4 proj_line_origin_inl(v3 a, v3 b) {
   Param4 res;
   res.p0 = res.p1 = res.p2 = res.p3 = 0;
   res.sqr_distance = -1;
@@ -479,7 +491,9 @@ HFB_HD_NOINLINE Param4 proj_line_origin(v3 a, v3 b) {
   }
   return res;
 }
-HFB_HD_NOINLINE Param4 proj_triangle_origin(v3 a, v3 b, v3 c) {
+HFB_HD_NOINLINE Param4 proj_line_origin(v3 a, v3 b) { return proj_line_origin_inl(a, b); }
+template <bool INL>
+HFB_HD Param4 proj_triangle_origin_inl(v3 a, v3 b, v3 c) {
   Param4 res;
   res.p0 = res.p1 = res.p2 = res.p3 = 0;
   res.sqr_distance = -1;
@@ -496,7 +510,7 @@ HFB_HD_NOINLINE Param4 proj_triangle_origin(v3 a, v3 b, v3 c) {
       if (dot(vi, cross(dli, n)) > 0) {
         const int j = i == 2 ? 0 : i + 1;
         const v3 vj = j == 0 ? a : (j == 1 ? b : c);
-        const Param4 rl = proj_line_origin(vi, vj);
+        const Param4 rl = INL ? proj_line_origin_inl(vi, vj) : proj_line_origin(vi, vj);
         if (mindist < 0 || rl.sqr_distance < mindist) {
           mindist = rl.sqr_distance;
           res.encode = (unsigned)(((rl.encode & 1) ? 1 << i : 0) + ((rl.encode & 2) ? 1 << j : 0));
@@ -520,6 +534,7 @@ HFB_HD_NOINLINE Param4 proj_triangle_origin(v3 a, v3 b, v3 c) {
   }
   return res;
 }
+HFB_HD_NOINLINE Param4 proj_triangle_origin(v3 a, v3 b, v3 c) { return proj_triangle_origin_inl<false>(a, b, c); }
 HFB_HD_NOINLINE Param4 proj_tetra_origin(v3 a, v3 b, v3 c, v3 d) {
   Param4 res;
   res.p0 = res.p1 = res.p2 = res.p3 = 0;
@@ -568,11 +583,13 @@ HFB_HD_NOINLINE Param4 proj_tetra_origin(v3 a, v3 b, v3 c, v3 d) {
 }
 
 // details::getClosestPoints (gjk.cpp:94-151) on a by-value simplex.  Most kernels call it out of line (closest_points);
-// one that inlines it keeps the simplex in registers (passed by reference to the call, it goes to local memory).
-HFB_HD void closest_points_inl(const SV& v0, const SV& v1, const SV& v2, const SV& v3_, int rank, v3& w0, v3& w1) {
+// one that inlines it keeps the simplex in registers (passed by reference to the call, it goes to local memory).  The
+// weights come from w alone; `st` hands each vertex's w0 / w1 to the sums (InRegs, or the passes' SlotStore).
+template <class Store = InRegs>
+HFB_HD void closest_points_inl(const typename Store::V& v0, const typename Store::V& v1, const typename Store::V& v2,
+                               const typename Store::V& v3_, int rank, v3& w0, v3& w1, const Store& st = Store()) {
   if (rank == 1) {
-    w0 = v0.w0;
-    w1 = v0.w1;
+    st.support_points(v0, w0, w1);
     return;
   }
   if (rank == 2) {
@@ -580,35 +597,42 @@ HFB_HD void closest_points_inl(const SV& v0, const SV& v1, const SV& v2, const S
     const v3 N = b - a;
     double la = dot(N, -a);
     if (la <= 0) {
-      w0 = v0.w0;
-      w1 = v0.w1;
+      st.support_points(v0, w0, w1);
     } else {
       double lb = sqn(N);
       if (la > lb) {
-        w0 = v1.w0;
-        w1 = v1.w1;
+        st.support_points(v1, w0, w1);
       } else {
         lb = la / lb;
         la = 1 - lb;
-        w0 = la * v0.w0 + lb * v1.w0;
-        w1 = la * v0.w1 + lb * v1.w1;
+        v3 a0, a1, b0, b1;
+        st.support_points(v0, a0, a1);
+        st.support_points(v1, b0, b1);
+        w0 = la * a0 + lb * b0;
+        w1 = la * a1 + lb * b1;
       }
     }
     return;
   }
   Param4 pr;
-  if (rank == 3) pr = proj_triangle_origin(v0.w, v1.w, v2.w);
+  if (rank == 3)
+    pr = Store::inline_projections ? proj_triangle_origin_inl<true>(v0.w, v1.w, v2.w) : proj_triangle_origin(v0.w, v1.w, v2.w);
   else pr = proj_tetra_origin(v0.w, v1.w, v2.w, v3_.w);
   // w0 = 0; w0 += p_i * vs[i].w0 ...
-  w0 = mk(0, 0, 0) + pr.p0 * v0.w0;
-  w1 = mk(0, 0, 0) + pr.p0 * v0.w1;
-  w0 = w0 + pr.p1 * v1.w0;
-  w1 = w1 + pr.p1 * v1.w1;
-  w0 = w0 + pr.p2 * v2.w0;
-  w1 = w1 + pr.p2 * v2.w1;
+  v3 s0, s1;
+  st.support_points(v0, s0, s1);
+  w0 = mk(0, 0, 0) + pr.p0 * s0;
+  w1 = mk(0, 0, 0) + pr.p0 * s1;
+  st.support_points(v1, s0, s1);
+  w0 = w0 + pr.p1 * s0;
+  w1 = w1 + pr.p1 * s1;
+  st.support_points(v2, s0, s1);
+  w0 = w0 + pr.p2 * s0;
+  w1 = w1 + pr.p2 * s1;
   if (rank == 4) {
-    w0 = w0 + pr.p3 * v3_.w0;
-    w1 = w1 + pr.p3 * v3_.w1;
+    st.support_points(v3_, s0, s1);
+    w0 = w0 + pr.p3 * s0;
+    w1 = w1 + pr.p3 * s1;
   }
 }
 HFB_HD_NOINLINE void closest_points(const SV& v0, const SV& v1, const SV& v2, const SV& v3_, int rank, v3& w0,
@@ -622,10 +646,11 @@ HFB_HD void inflate(const MinkD& md, v3 normal, v3& w0, v3& w1) {
   if (md.ssr1 > 0) w1 = w1 - md.ssr1 * normal;
 }
 
-// GJK::getWitnessPointsAndNormal (gjk.cpp:177-186); INL: closest_points inlined
-template <bool INL = false>
-HFB_HD void gjk_witness(const GjkState& g, const MinkD& md, v3& w0, v3& w1, v3& normal) {
-  if (INL) closest_points_inl(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1);
+// GJK::getWitnessPointsAndNormal (gjk.cpp:177-186); INL: closest_points inlined (a Store other than InRegs needs it)
+template <bool INL = false, class Store = InRegs>
+HFB_HD void gjk_witness(const GjkStateT<typename Store::V>& g, const MinkD& md, v3& w0, v3& w1, v3& normal,
+                        const Store& st = Store()) {
+  if constexpr (INL) closest_points_inl(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1, st);
   else closest_points(g.s0, g.s1, g.s2, g.s3, g.rank, w0, w1);
   if (nrm(w1 - w0) > HFB_DUMMY_PRECISION) normal = unit(w1 - w0);
   else normal = -unit(g.ray);

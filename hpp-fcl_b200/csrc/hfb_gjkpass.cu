@@ -7,21 +7,21 @@
 // a warp that keeps its 32 pairs until the last one has converged idles most of its lanes; and set-up, iteration
 // and witness extraction together are ~13 000 instructions against an instruction cache of 2 000 (32 KB L1.5 per
 // SM), with the warps of an SM spread all over them.  Here:
-//   k_gjk_first   set-up + the first K1 iterations of every pair            -> finished-pair or loop state to HBM
-//   k_gjk_more    K2, K3, ... more iterations of the pairs still running, which each pass compacts into a list
-//                 (the last pass runs to convergence)
-//   k_gjk_end     status machine + witness points of every pair: result record, or an EPA queue item
-// Every kernel is small, and the later passes run full warps of the long pairs.
+//   k_gjk_first<MODE>   set-up + the first K1 iterations of every pair; the loop state of the pairs still running to
+//                       HBM, and the pairs appended to a list
+//   k_gjk_more<MODE>    K2, K3, ... more iterations of the pairs still running, which each pass compacts into a list
+//                       (the last pass runs to convergence)
+// A pair whose iterations end is finished by the kernel that ran them: status machine + witness points (pair_gjk_end),
+// result record or EPA queue item.  Every kernel is small, and the later passes run full warps of the long pairs.
 //
-// The state between the kernels is stored field-major (one row per scalar field, one column per pair), so that the
-// lanes of a warp, which hold consecutive pairs, move consecutive words.  A finished pair leaves 52 B plus 48 B per
-// live simplex vertex (w = w0 - w1 is not stored: gjk_support computed it that way); a pair still running leaves its
-// loop state, 56 B plus 48 B per live vertex (plus 52 B for the Polyak and Nesterov variants), at its slot in the
-// list of running pairs, where the next pass reads it densely.
+// The loop state of a running pair is stored field-major (one row per scalar field, one column per slot in the list
+// of running pairs), so that the lanes of a warp, which hold consecutive slots, move consecutive words: 56 B plus 48 B
+// per live simplex vertex (plus 52 B for the Polyak and Nesterov variants), where the next pass reads it densely.
 //
 // Inside k_gjk_first and k_gjk_more a simplex vertex is w and a slot id (SVSlot): the support points w0 / w1, which
-// the iterations never read, wait in a per-thread store in shared memory (SlotStore) until the pair's state is saved.
-// That leaves registers for 3 blocks of 128 threads per SM instead of 2.
+// the iterations never read, wait in a per-thread store in shared memory (SlotStore) until the pair's loop state is
+// saved, its witness points are summed (their weights come from w) or its EPA item is written.  That leaves
+// registers for 3 blocks of 128 threads per SM instead of 2.
 #include "hfb_gjkpass.h"
 
 namespace {
@@ -33,6 +33,7 @@ enum { PASS_THREADS = 128, PASS_BLOCKS_PER_SM = 3 };  // k_gjk_first / k_gjk_mor
 // live vertex uses: at most 3 vertices are live when it appends, so one is always free.
 struct SlotStore {
   using V = SVSlot;
+  static constexpr bool inline_projections = true;  // (168 registers per thread)
   double* col;  // this thread's column: component c of slot j at col[(6 * j + c) * PASS_THREADS]
 
   __device__ __forceinline__ void st(int j, v3 w0, v3 w1) const {
@@ -61,13 +62,9 @@ struct SlotStore {
     put(g, g.rank, v);
     return nv.w;
   }
+  __device__ __forceinline__ void support_points(const SVSlot& v, v3& w0, v3& w1) const { ld(v.slot, w0, w1); }
 };
 
-#define HFB_GJK_UNKNOWN_TYPES (-99)  // status of a pair whose node types no kernel knows (reported as unsupported)
-
-// rows of the finished-pair state (by position in the class-sorted range)
-enum { FD_DIST = 0, FD_RAY = 1, FD_W = 4, FD_ROWS = FD_W + 4 * 6 };  // slot j: w0 xyz at FD_W + 6j, w1 xyz after
-enum { FI_STATUS = 0, FI_RANK, FI_ITER, FI_HINT0, FI_HINT1, FI_ROWS };
 // rows of the loop state of a running pair (by slot in the running list).  A pair that goes on into the next pass
 // has at most 3 live vertices: a rank-4 simplex either encloses the origin, which ends GJK, or is projected onto
 // one of its faces, edges or vertices.
@@ -80,10 +77,8 @@ struct Rows {  // entry `at` of row r: d[r * stride + at] / i[r * stride + at]
   int* i;
 };
 struct PassState {
-  Rows fin;              // finished pairs
-  unsigned char* done;   // per position: 1 finished in the first pass, 2 in a later pass, 0 running
-  Rows run[2];           // running pairs, two buffers, ping-ponged like the lists
-  size_t stride;         // positions of the range (rows of every buffer have this length)
+  Rows run[2];    // running pairs, two buffers, ping-ponged like the lists
+  size_t stride;  // positions of the range (rows of every buffer have this length)
 };
 
 struct PassArgs {
@@ -94,7 +89,6 @@ struct PassArgs {
   unsigned* out_count;
   Rows rin, rout;            // loop state of the pairs of in_list / out_list (entries of st.run)
   int steps;
-  int which;  // k_gjk_end: the pairs with this `done` value
 };
 
 __device__ __forceinline__ void st3r(double* d, size_t stride, int row, unsigned at, v3 v) {
@@ -104,55 +98,6 @@ __device__ __forceinline__ void st3r(double* d, size_t stride, int row, unsigned
 }
 __device__ __forceinline__ v3 ld3r(const double* d, size_t stride, int row, unsigned at) {
   return mk(d[row * stride + at], d[(row + 1) * stride + at], d[(row + 2) * stride + at]);
-}
-
-// what pair_gjk_end and push_epa_item read of a finished pair
-__device__ __forceinline__ void save_finished(const PassState& st, unsigned pos, const GjkStateT<SVSlot>& g,
-                                              const SlotStore& ss) {
-  const size_t m = st.stride;
-  int* fi = st.fin.i;
-  double* fd = st.fin.d;
-  fi[FI_STATUS * m + pos] = g.status;
-  fi[FI_RANK * m + pos] = g.rank;
-  fi[FI_ITER * m + pos] = (int)g.iterations;
-  fi[FI_HINT0 * m + pos] = g.hint0;
-  fi[FI_HINT1 * m + pos] = g.hint1;
-  fd[FD_DIST * m + pos] = g.distance;
-  st3r(fd, m, FD_RAY, pos, g.ray);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    if (j < g.rank) {
-      v3 w0, w1;
-      ss.ld(pick(g, j).slot, w0, w1);
-      st3r(fd, m, FD_W + 6 * j, pos, w0);
-      st3r(fd, m, FD_W + 6 * j + 3, pos, w1);
-    }
-  }
-}
-// the slots at and above `rank` are not stored; they are zero here (nothing reads them: the witness points use the
-// live ones, and EPA writes a slot before it raises the rank over it)
-__device__ __forceinline__ void load_finished(const PassState& st, unsigned pos, int status, GjkState& g) {
-  const size_t m = st.stride;
-  const int* fi = st.fin.i;
-  const double* fd = st.fin.d;
-  g.status = status;
-  g.rank = fi[FI_RANK * m + pos];
-  g.iterations = (unsigned)fi[FI_ITER * m + pos];
-  g.hint0 = fi[FI_HINT0 * m + pos];
-  g.hint1 = fi[FI_HINT1 * m + pos];
-  g.distance = fd[FD_DIST * m + pos];
-  g.ray = ld3r(fd, m, FD_RAY, pos);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    SV v;
-    v.w0 = v.w1 = v.w = mk(0, 0, 0);
-    if (j < g.rank) {
-      v.w0 = ld3r(fd, m, FD_W + 6 * j, pos);
-      v.w1 = ld3r(fd, m, FD_W + 6 * j + 3, pos);
-      v.w = v.w0 - v.w1;
-    }
-    put(g, j, v);
-  }
 }
 
 // the loop state of a pair that goes on into the next pass.  L.w and L.dir are only carried from one iteration to
@@ -219,6 +164,44 @@ __device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q
   }
 }
 
+// what load_pair_in and pair_gjk_begin leave in `o` for the extractors, read again when they run rather than kept
+// in registers across the iterations
+__device__ __forceinline__ PairOut begin_out(const BatchArgs& a, unsigned i) {
+  PairOut o;
+  o.cached_guess = mk(1, 0, 0);
+  o.hint0 = o.hint1 = 0;
+  o.iterations = 0;
+  if (a.P.initial_guess == HFB_GUESS_CACHED) {
+    if (a.guess_in) o.cached_guess = mk(a.guess_in[3 * i], a.guess_in[3 * i + 1], a.guess_in[3 * i + 2]);
+    if (a.hint_in) {
+      o.hint0 = a.hint_in[2 * i];
+      o.hint1 = a.hint_in[2 * i + 1];
+    }
+  }
+  return o;
+}
+
+// pair_gjk_end of a pair whose iterations ended: its EPA queue item, or its result record.  Of what make_setup<CAP_PRIM>
+// builds, the extractors read the first pose, `swapped` (false) and the two radii.  The radii are kept from the set-up
+// (reading them again costs two dependent loads, handle then shape record, on the pair's last step); the pose, which
+// the iterations do not need, is read again here rather than kept in registers.
+template <int MODE>
+__device__ __forceinline__ void finish_pair(const BatchArgs& a, unsigned i, GjkStateT<SVSlot>& g, const SlotStore& ss,
+                                            double ssr0, double ssr1) {
+  if (g.status == HFB_GJK_COLLISION && a.P.compute_penetration) {  // the EPA case of pair_gjk_end
+    push_epa_item(a, i, g, ss);
+    return;
+  }
+  GjkSetup S;
+  S.tfa = load_xf(a.tf1[i].R);
+  S.swapped = false;
+  S.md.ssr0 = ssr0;
+  S.md.ssr1 = ssr1;
+  PairOut o = begin_out(a, i);
+  pair_gjk_end<true>(a.P, S, g, o, ss);
+  store_result<MODE>(a, i, o);
+}
+
 // appends `pos` to the running list if `more`; returns its slot there
 __device__ __forceinline__ unsigned append_running(const PassArgs& p, bool more, unsigned pos) {
   const unsigned m = __ballot_sync(0xffffffffu, more);
@@ -232,6 +215,7 @@ __device__ __forceinline__ unsigned append_running(const PassArgs& p, bool more,
   return q;
 }
 
+template <int MODE>
 __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_first(const BatchArgs a, const PassArgs p) {
   __shared__ double store_rows[4 * 6 * PASS_THREADS];
   const SlotStore ss{store_rows + threadIdx.x};
@@ -240,31 +224,39 @@ __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_first(
   const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned k0 = lo + blockIdx.x * blockDim.x; k0 < hi; k0 += stride) {  // (warp-uniform trip count)
     const unsigned k = k0 + threadIdx.x;
-    bool more = false;
+    bool more = false, fin = false;
+    unsigned i = 0;
+    double ssr0 = 0, ssr1 = 0;
     GjkStateT<SVSlot> g;
     GjkLoop L;
     if (k < hi) {
-      const unsigned i = a.index_list[k];
+      i = a.index_list[k];
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       if (!type_known(in.s1.type) || !type_known(in.s2.type)) {
-        p.st.fin.i[FI_STATUS * p.st.stride + (k - lo)] = HFB_GJK_UNKNOWN_TYPES;
+        PairOut o = begin_out(a, i);
+        set_unsupported(o);
+        store_result<MODE>(a, i, o);
       } else {
         GjkSetup S;
         PairOut o;
         pair_gjk_begin<CAP_PRIM>(in, a.P, S, L, g, o);
+        ssr0 = S.md.ssr0;
+        ssr1 = S.md.ssr1;
         more = true;
         for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
-        if (!more) save_finished(p.st, k - lo, g, ss);
+        fin = !more;
       }
-      p.st.done[k - lo] = more ? 0 : 1;
     }
+    // the pairs that ended are finished after the others are saved: the loop state is dead by then
     if (p.out_list) {
       const unsigned q = append_running(p, more, k - lo);
       if (more) save_running(p.rout, p.st.stride, q, g, L, momentum, ss);
     }
+    if (fin) finish_pair<MODE>(a, i, g, ss, ssr0, ssr1);
   }
 }
 
+template <int MODE>
 __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_more(const BatchArgs a, const PassArgs p) {
   __shared__ double store_rows[4 * 6 * PASS_THREADS];
   const SlotStore ss{store_rows + threadIdx.x};
@@ -275,69 +267,27 @@ __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_more(c
   for (unsigned q0 = blockIdx.x * blockDim.x; q0 < n; q0 += stride) {
     const unsigned q = q0 + threadIdx.x;
     bool more = false;
-    unsigned pos = 0;
+    unsigned pos = 0, i = 0;
+    double ssr0 = 0, ssr1 = 0;
     GjkStateT<SVSlot> g;
     GjkLoop L;
     if (q < n) {
       pos = p.in_list[q];
-      const unsigned i = a.index_list[lo + pos];
+      i = a.index_list[lo + pos];
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       GjkSetup S;
       make_setup<CAP_PRIM>(in, S);
+      ssr0 = S.md.ssr0;
+      ssr1 = S.md.ssr1;
       load_running(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L, ss);
       more = true;
       for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
-      if (!more) {
-        save_finished(p.st, pos, g, ss);
-        p.st.done[pos] = 2;
-      }
     }
     if (p.out_list) {
       const unsigned qo = append_running(p, more, pos);
       if (more) save_running(p.rout, p.st.stride, qo, g, L, momentum, ss);
     }
-  }
-}
-
-template <int MODE>
-__global__ void __launch_bounds__(128) k_gjk_end(const BatchArgs a, const PassArgs p) {
-  const unsigned lo = *a.range_lo, hi = *a.range_hi;
-  for (unsigned k = lo + blockIdx.x * blockDim.x + threadIdx.x; k < hi; k += gridDim.x * blockDim.x) {
-    const unsigned pos = k - lo;
-    if (p.which >= 0 && p.st.done[pos] != p.which) continue;  // (which < 0: every pair, one launch after the last pass)
-    const unsigned i = a.index_list[k];
-    const int status = p.st.fin.i[FI_STATUS * p.st.stride + pos];
-    GjkState g;
-    if (status != HFB_GJK_UNKNOWN_TYPES) {
-      load_finished(p.st, pos, status, g);
-      if (status == HFB_GJK_COLLISION && a.P.compute_penetration) {  // the EPA case of pair_gjk_end
-        push_epa_item(a, i, g);
-        continue;
-      }
-    }
-    // what load_pair_in and pair_gjk_begin leave in `o` for the extractors
-    PairOut o;
-    o.cached_guess = mk(1, 0, 0);
-    o.hint0 = o.hint1 = 0;
-    o.iterations = 0;
-    if (a.P.initial_guess == HFB_GUESS_CACHED) {
-      if (a.guess_in) o.cached_guess = mk(a.guess_in[3 * i], a.guess_in[3 * i + 1], a.guess_in[3 * i + 2]);
-      if (a.hint_in) {
-        o.hint0 = a.hint_in[2 * i];
-        o.hint1 = a.hint_in[2 * i + 1];
-      }
-    }
-    if (status == HFB_GJK_UNKNOWN_TYPES) {
-      set_unsupported(o);
-    } else {
-      // of what make_setup<CAP_PRIM> builds, the extractors read the first pose, `swapped` and the two radii
-      GjkSetup S;
-      S.tfa = load_xf(a.tf1[i].R);
-      S.swapped = false;
-      mink_radii(load_shape<CAP_PRIM>(a.A, a.h1[i]), load_shape<CAP_PRIM>(a.A, a.h2[i]), S.md);
-      pair_gjk_end<true>(a.P, S, g, o);
-    }
-    store_result<MODE>(a, i, o);
+    if (q < n && !more) finish_pair<MODE>(a, i, g, ss, ssr0, ssr1);
   }
 }
 
@@ -350,9 +300,6 @@ size_t carve(void* base, size_t n, PassState& st) {
     return q;
   };
   st.stride = n;
-  st.fin.d = static_cast<double*>(take(FD_ROWS * n * sizeof(double)));
-  st.fin.i = static_cast<int*>(take(FI_ROWS * n * sizeof(int)));
-  st.done = static_cast<unsigned char*>(take(n));
   for (Rows& r : st.run) {
     r.d = static_cast<double*>(take(RD_ROWS * n * sizeof(double)));
     r.i = static_cast<int*>(take(RI_ROWS * n * sizeof(int)));
@@ -374,16 +321,11 @@ static unsigned pass_blocks(unsigned n, int num_sms) {
   if (blocks > cap) blocks = cap;
   return blocks ? blocks : 1u;
 }
-static void launch_end(const BatchArgs& a, int mode, PassArgs p, int which, unsigned blocks, cudaStream_t s) {
-  p.which = which;
-  if (mode == 0) k_gjk_end<0><<<blocks, 128, 0, s>>>(a, p);
-  else k_gjk_end<1><<<blocks, 128, 0, s>>>(a, p);
-}
 
-// first pass + extraction of the pairs it finished (their EPA items are in the queue when this returns, so that the
+// the first pass (the result records and EPA items of the pairs it finished are written when it ends, so that the
 // caller can start EPA on a side stream next to the remaining passes)
 int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, unsigned* counts,
-                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches, bool extract_now) {
+                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches) {
   if (npass < 1) return (int)cudaErrorInvalidValue;
   cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)npass * sizeof(unsigned), s);
   if (e != cudaSuccess) return (int)e;
@@ -396,28 +338,19 @@ int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint
   p.out_count = counts;
   p.rout = p.st.run[0];
   p.steps = npass > 1 ? steps[0] : 0x7fffffff;
-  p.which = 0;
-  k_gjk_first<<<blocks, PASS_THREADS, 0, s>>>(a, p);
-  // the pairs this pass finished are extracted now only when somebody waits for their EPA items (EPA on a side
-  // stream next to the remaining passes); otherwise one extraction launch after the last pass takes every pair, with
-  // full warps
-  if (extract_now || npass < 2) {
-    launch_end(a, mode, p, npass < 2 ? -1 : 1, blocks, s);
-    *launches += 1;
-  }
+  if (mode == 0) k_gjk_first<0><<<blocks, PASS_THREADS, 0, s>>>(a, p);
+  else k_gjk_first<1><<<blocks, PASS_THREADS, 0, s>>>(a, p);
   *launches += 1;
   return (int)cudaGetLastError();
 }
 
-// the remaining passes + extraction of the pairs they finished
+// the remaining passes
 int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, uint32_t* list_b,
-                    unsigned* counts, const int* steps, int npass, int num_sms, cudaStream_t s, int* launches,
-                    bool first_extracted) {
+                    unsigned* counts, const int* steps, int npass, int num_sms, cudaStream_t s, int* launches) {
   if (npass < 2) return 0;
   const unsigned blocks = pass_blocks(n, num_sms);
   PassArgs p;
   carve(state, n, p.st);
-  p.which = 0;
   for (int k = 1; k < npass; ++k) {
     const bool last = k + 1 == npass;
     // list_a goes with run[0], list_b with run[1]
@@ -433,10 +366,9 @@ int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint3
     const unsigned wave = (unsigned)num_sms * PASS_BLOCKS_PER_SM;
     unsigned b = blocks >> (k < 3 ? k : 3);
     if (b < wave) b = wave < blocks ? wave : blocks;
-    k_gjk_more<<<b, PASS_THREADS, 0, s>>>(a, p);
+    if (mode == 0) k_gjk_more<0><<<b, PASS_THREADS, 0, s>>>(a, p);
+    else k_gjk_more<1><<<b, PASS_THREADS, 0, s>>>(a, p);
     ++*launches;
   }
-  launch_end(a, mode, p, first_extracted ? 2 : -1, blocks, s);
-  ++*launches;
   return (int)cudaGetLastError();
 }

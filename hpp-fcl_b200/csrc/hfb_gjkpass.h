@@ -7,12 +7,11 @@
 // bytes of solver state for n pairs
 size_t gjk_pass_state_bytes(size_t n);
 // GJK over the class-sorted range [*a.range_lo, *a.range_hi) of a.index_list (at most n pairs) in `npass` passes of
-// steps[0], steps[1], ... iterations (the last pass runs to convergence).  gjk_passes_first: the first pass and the
-// extraction (result records, or EPA queue items) of the pairs it finished; gjk_passes_rest: the other passes and
-// the extraction of theirs.  Between the two the caller may start EPA over the queue so far on a side stream.
-// `counts`: npass words.  Return a cudaError_t as int.
+// steps[0], steps[1], ... iterations (the last pass runs to convergence).  Every pass writes the result records, or
+// EPA queue items, of the pairs it finished.  gjk_passes_first: the first pass; gjk_passes_rest: the other passes.
+// Between the two the caller may start EPA over the queue so far on a side stream.  `counts`: npass words.  Return a
+// cudaError_t as int.
 int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, unsigned* counts,
-                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches, bool extract_now);
+                     const int* steps, int npass, int num_sms, cudaStream_t s, int* launches);
 int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, uint32_t* list_b,
-                    unsigned* counts, const int* steps, int npass, int num_sms, cudaStream_t s, int* launches,
-                    bool first_extracted);
+                    unsigned* counts, const int* steps, int npass, int num_sms, cudaStream_t s, int* launches);

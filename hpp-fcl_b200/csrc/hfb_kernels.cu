@@ -303,8 +303,9 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
     k = __shfl_sync(Coop<G>::mask(), k, (threadIdx.x & 31u) & ~(unsigned)(G - 1));
     if (k >= hi) break;
     const unsigned k_pos = k;  // (tier 1: position in the retry list = slot of the continuation record)
-    // tier 0 hands the queue out from its end: k_gjk_end fills it in pair-class order, with the cylinder classes last.
-    // Their runs are the longest, so starting them first shortens the end of the launch
+    // tier 0 hands the queue out from its end: the first GJK pass fills it in pair-class order, with the cylinder
+    // classes last, and the later passes append the pairs whose GJK ran longer.  Their runs are the longest, so starting
+    // them first shortens the end of the launch
     if (TIER == 0) k = lo + hi - 1 - k;
     if (TIER == 1) k = a.retry[k];
     const EpaItem* it = a.queue + k;
@@ -1153,7 +1154,7 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
           {
             KTimer kt(ctx, ws, 0);
             if (gjk_passes_first(ag, MODE, n, sl.gstate.p, la, static_cast<unsigned*>(sl.gcnt.p), ctx->gjk_steps, ctx->gjk_npass,
-                                 ctx->num_sms, ws, &nl, early_epa) != 0)
+                                 ctx->num_sms, ws, &nl) != 0)
               return fail(ctx, HFB_ERR_CUDA, "GJK pass launch failed");
           }
           // EPA of the pairs the first pass finished starts on the side stream, next to the remaining passes (which
@@ -1162,7 +1163,7 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
           {
             KTimer kt(ctx, ws, 0);
             if (gjk_passes_rest(ag, MODE, n, sl.gstate.p, la, la + n, static_cast<unsigned*>(sl.gcnt.p), ctx->gjk_steps,
-                                ctx->gjk_npass, ctx->num_sms, ws, &nl, early_epa) != 0)
+                                ctx->gjk_npass, ctx->num_sms, ws, &nl) != 0)
               return fail(ctx, HFB_ERR_CUDA, "GJK pass launch failed");
           }
           ctx->stats.kernel_launches += (uint64_t)nl;

@@ -150,9 +150,10 @@ HFB_HD void pair_gjk_begin(const PairIn& in, const SolverP& P, GjkSetup& S, GjkL
   const v3 guess = initial_guess(P, in, S);
   gjk_begin(S.md, P.gjk, guess, in.hint0, in.hint1, g, L);
 }
-// returns true when EPA must still run (g holds GJK's final simplex); INL: see gjk_witness
-template <bool INL = false>
-HFB_HD bool pair_gjk_end(const SolverP& P, const GjkSetup& S, GjkState& g, PairOut& o) {
+// returns true when EPA must still run (g holds GJK's final simplex); INL, st: see gjk_witness
+template <bool INL = false, class Store = InRegs>
+HFB_HD bool pair_gjk_end(const SolverP& P, const GjkSetup& S, GjkStateT<typename Store::V>& g, PairOut& o,
+                         const Store& st = Store()) {
   o.iterations = g.iterations & 0xffffu;
   o.status = pack_status(g.status, HFB_EPA_DID_NOT_RUN, HFB_PATH_GJK);
   switch (g.status) {
@@ -163,7 +164,7 @@ HFB_HD bool pair_gjk_end(const SolverP& P, const GjkSetup& S, GjkState& g, PairO
       o.hint0 = g.hint0;
       o.hint1 = g.hint1;
       o.distance = g.distance;
-      gjk_witness<INL>(g, S.md, o.p1, o.p2, o.normal);
+      gjk_witness<INL>(g, S.md, o.p1, o.p2, o.normal, st);
       recentre(S.tfa, o.distance, o.p1, o.p2, o.normal);
       unswap(S, o);
     } break;
