@@ -73,14 +73,11 @@ struct EpaParams {
   unsigned max_iterations;
 };
 
+// The counters and the status of a run.  The result (normal, depth, the three vertices of the closest face, the
+// iteration count) is not kept here: it is read from EpaLoop and the workspace once the run is over (pair_epa_result).
 struct EpaState {
   int status;       // EPA::Status value
-  v3 normal;
-  double depth;
-  int rank;         // result.rank (3, or 1 on FallBack)
-  SV r0, r1, r2;    // result.vertex[0..2]
   int hint0, hint1;
-  unsigned iterations;
   // bookkeeping
   int num_vertices, hull_count, stock_top, seq;  // stock_top: freed slots waiting in EpaWs::stock
   int hwm;        // slots [0, hwm) have been handed out at least once
@@ -90,14 +87,6 @@ struct EpaState {
 
 template <class WS>
 HFB_HD v3 ws_vw(const WS* ws, int i) { return mk(ws->vw[3 * i], ws->vw[3 * i + 1], ws->vw[3 * i + 2]); }
-template <class WS>
-HFB_HD SV ws_sv(const WS* ws, int i) {
-  SV s;
-  s.w0 = mk(ws->vw0[3 * i], ws->vw0[3 * i + 1], ws->vw0[3 * i + 2]);
-  s.w1 = mk(ws->vw1[3 * i], ws->vw1[3 * i + 1], ws->vw1[3 * i + 2]);
-  s.w = ws_vw(ws, i);
-  return s;
-}
 template <class WS>
 HFB_HD void ws_put_v(WS* ws, int i, const SV& s) {
   ws->vw0[3 * i] = s.w0.x;
@@ -427,9 +416,6 @@ HFB_HD bool epa_begin(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const
   const double tol = P.tolerance;
   E.hint0 = g.hint0;
   E.hint1 = g.hint1;
-  E.iterations = 0;
-  E.depth = 0;
-  E.normal = mk(0, 0, 0);
   E.nverts_cap = P.max_iterations + 4;
   E.nfaces_cap = 2 * P.max_iterations + 4;
   L.it = 0;
@@ -481,11 +467,9 @@ HFB_HD bool epa_begin(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const
       return true;
     }
   }
-  // FallBack (:1299-1315); the solver maps it to EPAFailedExtract... (narrowphase.h:574-582)
+  // FallBack (:1299-1315); the solver maps it to EPAFailedExtract... (narrowphase.h:574-582), which reads neither the
+  // depth nor the result vertex (g.s0) the reference sets here
   E.status = HFB_EPA_FALLBACK;
-  E.depth = 0;
-  E.rank = 1;
-  E.r0 = g.s0;
   return false;
 }
 
@@ -557,28 +541,21 @@ HFB_HD void epa_run(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const E
   L.closest = closest;
 }
 
-// part 3: the result (:1291-1298)
-template <class WS>
-HFB_HD void epa_finish(const MinkD& md, const EpaParams& P, const WS* ws, EpaState& E, const EpaLoop& L) {
-  E.iterations = L.it;
+// part 3: the final status (:1291-1298).  The rest of the result is that of the last good closest face: its normal
+// and offset in L (outer_n, outer_d), its vertices (result.vertex[0..2]) at L.ov0..2 in the workspace, the iteration
+// count in L.it; the depth is outer_d plus the two radii (epa_depth).
+HFB_HD void epa_finish(const EpaParams& P, EpaState& E, const EpaLoop& L) {
   if (!(L.it < P.max_iterations)) E.status = HFB_EPA_FAILED;
-  E.normal = L.outer_n;
-  E.depth = L.outer_d + (md.ssr0 + md.ssr1);
-  E.rank = 3;
-  E.r0 = ws_sv(ws, L.ov0);
-  E.r1 = ws_sv(ws, L.ov1);
-  E.r2 = ws_sv(ws, L.ov2);
 }
+HFB_HD double epa_depth(const MinkD& md, const EpaLoop& L) { return L.outer_d + (md.ssr0 + md.ssr1); }
 
 template <int G, int CAPS, class WS>
 HFB_HD void epa_evaluate(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const EpaParams& P, GjkState& g, WS* ws,
-                         EpaState& E, EpaLoop* Lout = nullptr) {
-  EpaLoop L;
+                         EpaState& E, EpaLoop& L) {
   if (epa_begin<G, CAPS>(sa, sb, md, P, g, ws, E, L)) {
     epa_run<G, CAPS>(sa, sb, md, P, ws, E, L);
-    if (!(E.status == HFB_EPA_WS_OVERFLOW && L.resumable)) epa_finish(md, P, ws, E, L);
+    if (!(E.status == HFB_EPA_WS_OVERFLOW && L.resumable)) epa_finish(P, E, L);
   }
-  if (Lout) *Lout = L;
 }
 
 // the live part of a workspace copied into a larger one (same slot and vertex numbers), by the G lanes of the group:
@@ -612,15 +589,38 @@ HFB_HD void epa_ws_grow(const WSA* a, WSB* b, const EpaState& E) {
   Coop<G>::sync();
 }
 
-// EPA::getWitnessPointsAndNormal (:1451-1466)
-HFB_HD void epa_witness(const EpaState& E, const MinkD& md, v3& w0, v3& w1, v3& normal) {
-  SV dummy = E.r0;
-  closest_points(E.r0, E.r1, E.r2, dummy, E.rank, w0, w1);
+// the support points of a result vertex, read from the workspace (the store closest_points_inl sums them from; the
+// vertex is its w and its id in the workspace)
+template <class WS>
+struct WsStore {
+  using V = SVSlot;
+  static constexpr bool inline_projections = false;
+  const WS* ws;
+  HFB_HD void support_points(const SVSlot& v, v3& w0, v3& w1) const {
+    w0 = mk(ws->vw0[3 * v.slot], ws->vw0[3 * v.slot + 1], ws->vw0[3 * v.slot + 2]);
+    w1 = mk(ws->vw1[3 * v.slot], ws->vw1[3 * v.slot + 1], ws->vw1[3 * v.slot + 2]);
+  }
+};
+
+// EPA::getWitnessPointsAndNormal (:1451-1466) of a finished run (not FallBack): the result simplex is the closest
+// face's three vertices, read from the workspace where the run left them.  Inlined, with the vertices passed by value:
+// handed by reference to the out-of-line closest_points, they would go through local memory.
+template <class WS>
+HFB_HD void epa_witness(const WS* ws, const EpaLoop& L, double depth, const MinkD& md, v3& w0, v3& w1, v3& normal) {
+  SVSlot r0, r1, r2;
+  r0.w = ws_vw(ws, L.ov0);
+  r0.slot = L.ov0;
+  r1.w = ws_vw(ws, L.ov1);
+  r1.slot = L.ov1;
+  r2.w = ws_vw(ws, L.ov2);
+  r2.slot = L.ov2;
+  const WsStore<WS> st = {ws};
+  closest_points_inl(r0, r1, r2, r0, 3, w0, w1, st);
   if (nrm(w0 - w1) > HFB_DUMMY_PRECISION) {
-    if (E.depth >= 0) normal = unit(w0 - w1);
+    if (depth >= 0) normal = unit(w0 - w1);
     else normal = unit(w1 - w0);
   } else {
-    normal = E.normal;
+    normal = L.outer_n;
   }
   inflate(md, normal, w0, w1);
 }

@@ -310,7 +310,10 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
     if (TIER == 1) k = a.retry[k];
     const EpaItem* it = a.queue + k;
     const unsigned i = it->pair;
-    const PairIn in = load_pair_in<CAPS>(a, i);
+    // the loop needs the two shapes and the Minkowski set-up only; the pose the witness points are mapped back with
+    // is read again when the run is over instead of being kept in registers across the loop
+    GjkSetup S;
+    make_setup<CAPS>(load_pair_in<CAPS>(a, i), S);
     GjkState g;
     g.rank = it->rank;
     g.hint0 = it->hint0;
@@ -331,17 +334,12 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
     g.s1.w = g.s1.w0 - g.s1.w1;
     g.s2.w = g.s2.w0 - g.s2.w1;
     g.s3.w = g.s3.w0 - g.s3.w1;
-    PairOut o;
-    o.cached_guess = mk(1, 0, 0);
-    o.hint0 = o.hint1 = 0;
     Coop<G>::sync();
+    EpaResume rs;
+    bool done;
     if (TIER == 0) {
-      EpaResume rs;
-      rs.L.resumable = 0;
-      const bool done = pair_phase2<G, CAPS>(in, a.P, g, ws, o, &rs);
-      if (done) {
-        if (Coop<G>::lane() == 0) store_result<MODE>(a, i, o);
-      } else {
+      done = pair_epa<G, CAPS>(S, a.P, g, ws, rs);
+      if (!done) {
         unsigned r = 0;
         if (Coop<G>::lane() == 0) {
           r = atomicAdd(a.retry_count, 1u);
@@ -356,15 +354,20 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
       }
     } else {
       const unsigned kk = k_pos;
-      bool done = false;
       if (a.cont && kk < a.cont_cap && a.cont[kk].rs.L.resumable) {
-        EpaResume rs = a.cont[kk].rs;
+        rs = a.cont[kk].rs;
         epa_ws_grow<G>(&a.cont[kk].ws, ws, rs.E);
-        done = pair_phase2_resume<G, CAPS>(in, a.P, g, ws, rs, o);
+        done = pair_epa_resume<G, CAPS>(S, a.P, ws, rs);
       } else {
-        done = pair_phase2<G, CAPS>(in, a.P, g, ws, o);
+        done = pair_epa<G, CAPS>(S, a.P, g, ws, rs);
       }
-      if (done && Coop<G>::lane() == 0) store_result<MODE>(a, i, o);
+    }
+    if (done) {
+      // make_setup's tfa: the first pose, or the second one when the operands were swapped (a triangle first)
+      S.tfa = load_xf((S.swapped ? a.tf2 : a.tf1)[i].R);
+      PairOut o;
+      pair_epa_result(S, g.iterations, rs, ws, o);
+      if (Coop<G>::lane() == 0) store_result<MODE>(a, i, o);
     }
     Coop<G>::sync();
   }

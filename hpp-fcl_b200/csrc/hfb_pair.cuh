@@ -292,62 +292,70 @@ HFB_HD bool pair_phase1(const PairIn& in, const SolverP& P, PairOut& o, GjkState
 }
 
 // ---- phase 2: EPA + EPAExtractWitnessPointsAndNormal (narrowphase.h:514-583, 658-723)
-// the result record of a finished EPA run
-HFB_HD void pair_epa_result(const GjkSetup& S, const GjkState& g, const EpaState& E, PairOut& o) {
-  o.iterations = (g.iterations & 0xffffu) | ((E.iterations & 0xffffu) << 16);
-  o.status = pack_status(HFB_GJK_COLLISION, E.status, HFB_PATH_GJK);
-  if (E.status == HFB_EPA_FALLBACK) {  // EPAFailedExtract... :713-723
+// what a run that outgrew a reduced-size workspace hands to its continuation in the full-size one
+struct EpaResume {
+  EpaState E;
+  EpaLoop L;
+};
+// the result record of a finished EPA run (r) whose workspace is `ws`.  Of S it reads the radii, tfa and swapped.
+template <class WS>
+HFB_HD void pair_epa_result(const GjkSetup& S, unsigned gjk_iterations, const EpaResume& r, const WS* ws, PairOut& o) {
+  o.iterations = (gjk_iterations & 0xffffu) | ((r.L.it & 0xffffu) << 16);
+  o.status = pack_status(HFB_GJK_COLLISION, r.E.status, HFB_PATH_GJK);
+  if (r.E.status == HFB_EPA_FALLBACK) {  // EPAFailedExtract... :713-723
     o.cached_guess = mk(1, 0, 0);
     o.hint0 = o.hint1 = 0;
     o.distance = -DBL_MAX;
     o.p1 = o.p2 = o.normal = nan3();
     return;
   }
-  o.cached_guess = -(E.depth * E.normal);
-  o.hint0 = E.hint0;
-  o.hint1 = E.hint1;
-  o.distance = fmin(0., -E.depth);
-  epa_witness(E, S.md, o.p1, o.p2, o.normal);
+  const double depth = epa_depth(S.md, r.L);
+  o.cached_guess = -(depth * r.L.outer_n);
+  o.hint0 = r.E.hint0;
+  o.hint1 = r.E.hint1;
+  o.distance = fmin(0., -depth);
+  epa_witness(ws, r.L, depth, S.md, o.p1, o.p2, o.normal);
   recentre(S.tfa, o.distance, o.p1, o.p2, o.normal);
   unswap(S, o);
 }
-// what a run that outgrew a reduced-size workspace hands to its continuation in the full-size one
-struct EpaResume {
-  EpaState E;
-  EpaLoop L;
-};
-// Returns false (and leaves `o` unset) only when WS is a reduced-size workspace and the polytope outgrew it.  With
-// `rs` given and rs->L.resumable set on return, (rs, *ws) is the state at the top of the iteration that did not fit:
-// pair_phase2_resume continues from a copy of it (epa_ws_grow); otherwise the caller runs the pair again, from the
+// EPA from GJK's final simplex `g`, up to the result record.  Returns false only when WS is a reduced-size workspace
+// and the polytope outgrew it; with r.L.resumable set, (r, *ws) is then the state at the top of the iteration that did
+// not fit, which pair_epa_resume continues from a copy of (epa_ws_grow); otherwise the pair is run again, from the
 // queued GJK state, in the full-size workspace.
+template <int G, int CAPS, class WS>
+HFB_HD bool pair_epa(const GjkSetup& S, const SolverP& P, GjkState& g, WS* ws, EpaResume& r) {
+  epa_evaluate<G, CAPS>(S.a, S.b, S.md, P.epa, g, ws, r.E, r.L);
+  return r.E.status != HFB_EPA_WS_OVERFLOW;
+}
+// the rest of a run that stopped with r.L.resumable set; `ws` holds the grown copy of its workspace
+template <int G, int CAPS, class WS>
+HFB_HD bool pair_epa_resume(const GjkSetup& S, const SolverP& P, WS* ws, EpaResume& r) {
+  epa_run<G, CAPS>(S.a, S.b, S.md, P.epa, ws, r.E, r.L);
+  if (r.E.status == HFB_EPA_WS_OVERFLOW && r.L.resumable) return false;  // (cannot happen in the full-size workspace)
+  epa_finish(P.epa, r.E, r.L);
+  return r.E.status != HFB_EPA_WS_OVERFLOW;
+}
+// pair_epa + the result record.  Returns false (and leaves `o` unset) only when WS is a reduced-size workspace and the
+// polytope outgrew it; `rs`, if given, then receives the state to resume from (see pair_epa).
 template <int G, int CAPS, class WS>
 HFB_HD bool pair_phase2(const PairIn& in, const SolverP& P, GjkState& g, WS* ws, PairOut& o, EpaResume* rs = nullptr) {
   GjkSetup S;
   make_setup<CAPS>(in, S);
-  EpaState E;
-  EpaLoop L;
-  epa_evaluate<G, CAPS>(S.a, S.b, S.md, P.epa, g, ws, E, &L);
-  if (E.status == HFB_EPA_WS_OVERFLOW) {
-    if (rs) {
-      rs->E = E;
-      rs->L = L;
-    }
+  EpaResume r;
+  if (!pair_epa<G, CAPS>(S, P, g, ws, r)) {
+    if (rs) *rs = r;
     return false;
   }
-  pair_epa_result(S, g, E, o);
+  pair_epa_result(S, g.iterations, r, ws, o);
   return true;
 }
-// the rest of a run that stopped with rs.L.resumable set; `ws` holds the grown copy of its workspace and `g` the GJK
-// iteration count of the pair (all the result record takes from it)
+// pair_epa_resume + the result record; `g` holds the GJK iteration count of the pair (all the record takes from it)
 template <int G, int CAPS, class WS>
 HFB_HD bool pair_phase2_resume(const PairIn& in, const SolverP& P, const GjkState& g, WS* ws, EpaResume& rs, PairOut& o) {
   GjkSetup S;
   make_setup<CAPS>(in, S);
-  epa_run<G, CAPS>(S.a, S.b, S.md, P.epa, ws, rs.E, rs.L);
-  if (rs.E.status == HFB_EPA_WS_OVERFLOW && rs.L.resumable) return false;  // (cannot happen in the full-size workspace)
-  epa_finish(S.md, P.epa, ws, rs.E, rs.L);
-  if (rs.E.status == HFB_EPA_WS_OVERFLOW) return false;
-  pair_epa_result(S, g, rs.E, o);
+  if (!pair_epa_resume<G, CAPS>(S, P, ws, rs)) return false;
+  pair_epa_result(S, g.iterations, rs, ws, o);
   return true;
 }
 
