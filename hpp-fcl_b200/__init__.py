@@ -9,7 +9,9 @@ raises if the extension or a GPU is missing.
 from . import _pod  # noqa: F401
 from ._pod import *  # noqa: F401,F403
 from .build import build_extension, library_path  # noqa: F401
-from .engine import Engine, EngineError, broadphase_pairs, build_bvh_obbrss, load_library  # noqa: F401
+from .engine import (  # noqa: F401
+    Engine, EngineError, broadphase_cross_pairs, broadphase_pairs, build_bvh_obbrss, load_library,
+)
 from .api import (  # noqa: F401
     BVHModelOBB, BVHModelOBBRSS, Box, Capsule, CollisionRequest, CollisionResult, Cone, Contact, Convex, Cylinder,
     DistanceRequest, DistanceResult, Ellipsoid, Halfspace, Plane, Sphere, Transform3f, TriangleP,

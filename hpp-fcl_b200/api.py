@@ -571,27 +571,73 @@ class DynamicAABBTreeCollisionManager:
     def update(self):
         self._refresh()
 
-    def pairs(self):
-        """the candidate pairs as object indices (first < second)"""
+    def _table(self, other):
+        """(handles, poses, boxes, objects) of `other`: another manager (refreshed if stale) or one CollisionObject,
+        whose box is computed here as setup() computes the manager's"""
+        if isinstance(other, DynamicAABBTreeCollisionManager):
+            if other._stale:
+                other._refresh()
+            return other._handles, other._tfs, other._boxes, other.objs
+        h = np.array([self.scene.handle(other.geom)], dtype=np.uint32)
+        self.scene.commit()
+        tf = _tf_array([other.tf])
+        bb = self.scene.engine.scene_aabbs(h, tf)
+        other.aabb = AABB(bb[0, :3].copy(), bb[0, 3:].copy())
+        return h, tf, bb, [other]
+
+    def _cross(self, other):
+        """-> (first, second, other's table): the cross candidates of this manager against `other` (a manager or a
+        CollisionObject), first in this manager, second in `other`; other's table computed once"""
+        if self._stale:
+            self._refresh()
+        from .engine import broadphase_cross_pairs
+        table = self._table(other)
+        first, second = broadphase_cross_pairs(self._boxes, table[2])
+        return first, second, table
+
+    def pairs(self, other=None):
+        """the candidate pairs as object indices: first < second in this manager; or, with `other` (a manager or a
+        CollisionObject), first in this manager and second in `other`"""
+        if other is not None and other is not self:
+            return self._cross(other)[:2]
         if self._stale:
             self._refresh()
         from .engine import broadphase_pairs
         return broadphase_pairs(self._boxes)
 
-    def collide(self, callback):
+    def collide(self, other=None, callback=None):
+        """collide(callback): every pair of this manager's objects with overlapping boxes.  collide(other, callback):
+        o1 from this manager, o2 from `other`, another manager (collide(self, cb) is the self form) or one
+        CollisionObject -- o2 is then that object, the order of DynamicAABBTreeCollisionManager::collide(obj)
+        (broadphase_dynamic_AABB_tree.cpp:361-390; NaiveCollisionManager passes (obj, object) instead)"""
+        if callback is None:  # collide(cb) / collide(callback=cb)
+            other, callback = None, other
         callback.init()
-        first, second = self.pairs()
+        if other is None or other is self:
+            first, second = self.pairs()
+            objs_b = self.objs
+        else:
+            first, second, table = self._cross(other)
+            objs_b = table[3]
         for a, b in zip(first.tolist(), second.tolist()):
-            if callback(self.objs[a], self.objs[b]):
+            if callback(self.objs[a], objs_b[b]):
                 return
 
-    def collide_batch(self, request=None):
-        """-> (first, second, contact records) of ALL candidate pairs: one hfb_batch_collide_objects call"""
+    def collide_batch(self, request=None, other=None):
+        """-> (first, second, contact records) of ALL candidate pairs: one hfb_batch_collide_objects call.  With
+        `other` (a manager or a CollisionObject): the cross pairs, o1 from this manager, o2 from `other`, over the
+        object table [this manager; other]"""
         request = request or CollisionRequest()
         if request.num_max_contacts == 0:
             raise ValueError("Invalid number of max contacts (current value is 0).")
-        first, second = self.pairs()
-        rec = self.scene.engine.batch_collide_objects(self._handles, self._tfs, first, second, request._pod)
+        if other is None or other is self:
+            first, second = self.pairs()
+            rec = self.scene.engine.batch_collide_objects(self._handles, self._tfs, first, second, request._pod)
+            return first, second, rec
+        first, second, (hb, tb, _, _) = self._cross(other)
+        n = len(self._handles)
+        rec = self.scene.engine.batch_collide_objects(np.concatenate([self._handles, hb]), np.concatenate([self._tfs, tb]),
+                                                      first, second + np.uint32(n), request._pod)
         return first, second, rec
 
 

@@ -112,26 +112,17 @@ __global__ void __launch_bounds__(256) k_make_grid(const Bounds* part, unsigned 
         v.lo[k] = v.hi[k] = 0;
       }
     }
-    double cell = v.ext > 0 ? v.ext : 1.0;
-    for (;;) {
-      double cells = 1;
-      for (int k = 0; k < 3; ++k) {
-        g.dim[k] = (int)floor((v.hi[k] - v.lo[k]) / cell) + 1;
-        cells *= g.dim[k];
-      }
-      if (cells <= (double)kMaxCells) break;
-      cell *= 1.26;
-    }
-    for (int k = 0; k < 3; ++k) g.origin[k] = v.lo[k];
-    g.inv_cell = 1.0 / cell;
+    grid_fit(v.lo, v.hi, v.ext > 0 ? v.ext : 1.0, g);
     *grid = g;
     *n_pairs = 0u;
     *n_unbounded = 0u;
   }
 }
-// cell of every object; the unbounded ones (cell 0xfffffffe) are listed from the END of `order` backwards
+// cell of every object; the unbounded ones (cell 0xfffffffe) are listed from the END of `order` backwards.
+// max_ext (cross form only, else null): boxes wider than *max_ext are listed with the unbounded ones
 __global__ void __launch_bounds__(256) k_cell_hist(const double* bb, unsigned n, const BroadGrid* grid, unsigned* cell,
-                                                   unsigned* count, unsigned* order, unsigned* n_unbounded) {
+                                                   unsigned* count, unsigned* order, unsigned* n_unbounded,
+                                                   const double* max_ext) {
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double* b = bb + 6 * (size_t)i;
@@ -139,7 +130,7 @@ __global__ void __launch_bounds__(256) k_cell_hist(const double* bb, unsigned n,
     cell[i] = 0xffffffffu;  // empty box: in no cell
     return;
   }
-  if (aabb_unbounded(b)) {
+  if (aabb_unbounded(b) || (max_ext && box_extent(b) > *max_ext)) {
     cell[i] = 0xfffffffeu;
     order[n - 1u - atomicAdd(n_unbounded, 1u)] = i;
     return;
@@ -241,6 +232,138 @@ __global__ void __launch_bounds__(128) k_sweep_unbounded(const double* bb, unsig
   }
 }
 
+// ---- cross form (design: hfb_broadphase.cuh, broadphase_cross_pairs_host) -------------------------------------
+struct CrossGrid {  // B's grid and its cell size (the largest extent a box in the grid may have)
+  BroadGrid g;
+  double cell;
+};
+
+// one warp's hits appended with one counter bump; every lane of the warp must call it
+__device__ __forceinline__ void append_pair(bool hit, unsigned a, unsigned b, uint32_t* first, uint32_t* second,
+                                            unsigned capacity, unsigned* n_pairs) {
+  const unsigned m = __ballot_sync(0xffffffffu, hit);
+  if (!m) return;
+  const unsigned lane = threadIdx.x & 31u;
+  unsigned base = 0;
+  if (lane == (unsigned)(__ffs(m) - 1)) base = atomicAdd(n_pairs, (unsigned)__popc(m));
+  base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
+  const unsigned pos = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+  if (hit && pos < capacity) {
+    first[pos] = a;
+    second[pos] = b;
+  }
+}
+
+// B's centres box and the log2 histogram of B's extents (bounded, non-empty boxes)
+__global__ void __launch_bounds__(256) k_cross_bounds_partial(const double* bb, unsigned n, Bounds* part, unsigned* hist) {
+  __shared__ unsigned sh_hist[kExtBins];
+  for (unsigned k = threadIdx.x; k < (unsigned)kExtBins; k += blockDim.x) sh_hist[k] = 0;
+  __syncthreads();
+  Bounds v = bounds_empty();
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const double* b = bb + 6 * (size_t)i;
+    if (aabb_empty(b) || aabb_unbounded(b)) continue;
+    Bounds o;
+    for (int k = 0; k < 3; ++k) o.lo[k] = o.hi[k] = 0.5 * (b[k] + b[3 + k]);
+    o.ext = 0;
+    bounds_merge(v, o);
+    atomicAdd(sh_hist + extent_bin(box_extent(b)), 1u);
+  }
+  v = block_bounds(v);  // (synchronises the block: the histogram is complete after it)
+  if (threadIdx.x == 0) part[blockIdx.x] = v;
+  for (unsigned k = threadIdx.x; k < (unsigned)kExtBins; k += blockDim.x)
+    if (sh_hist[k]) atomicAdd(hist + k, sh_hist[k]);
+}
+// one block: final merge, the cell from the histogram, the grid, and the zeroed counters (pairs, B oversize, A brute)
+__global__ void __launch_bounds__(256) k_cross_grid(const Bounds* part, unsigned nparts, const unsigned* hist, CrossGrid* cg,
+                                                    unsigned* n_pairs, unsigned* counters) {
+  Bounds v = bounds_empty();
+  for (unsigned i = threadIdx.x; i < nparts; i += blockDim.x) bounds_merge(v, part[i]);
+  v = block_bounds(v);
+  if (threadIdx.x == 0) {
+    unsigned total = 0;
+    for (int k = 0; k < kExtBins; ++k) total += hist[k];
+    if (!(v.lo[0] <= v.hi[0]))
+      for (int k = 0; k < 3; ++k) v.lo[k] = v.hi[k] = 0;
+    CrossGrid c;
+    c.cell = cross_grid_fit(v.lo, v.hi, hist, total, c.g);
+    *cg = c;
+    *n_pairs = 0u;
+    counters[0] = counters[1] = 0u;
+  }
+}
+// one A object per thread, i in [a_lo, a_hi): the B objects in the grid rows its widened box covers, then B's oversize
+// and unbounded ones (listed from the end of `order`); A objects that need the whole of B are listed in `brute`
+__global__ void __launch_bounds__(128) k_cross_sweep(const double* ba, unsigned a_lo, unsigned a_hi, const double* bb,
+                                                     unsigned nb, const CrossGrid* cgp, const unsigned* start,
+                                                     const unsigned* order, unsigned* counters, unsigned* brute,
+                                                     uint32_t* first, uint32_t* second, unsigned second_base,
+                                                     unsigned capacity, unsigned* n_pairs) {
+  const unsigned i = a_lo + blockIdx.x * blockDim.x + threadIdx.x;
+  const CrossGrid cg = *cgp;
+  bool live = i < a_hi && !aabb_empty(ba + 6 * (size_t)i);
+  double mine[6] = {0, 0, 0, 0, 0, 0};
+  int c0[3] = {0, 0, 0}, c1[3] = {-1, -1, -1};
+  if (live) {
+    for (int k = 0; k < 6; ++k) mine[k] = ba[6 * (size_t)i + k];
+    if (aabb_unbounded(mine) || cross_query_cells(cg.g, cg.cell, mine, c0, c1) > kCrossScanRows) {
+      brute[atomicAdd(counters + 1, 1u)] = i;
+      live = false;
+    }
+  }
+  // the lanes walk their rows side by side: a lane whose row is done fetches its next one
+  int y = c0[1], z = c0[2];
+  unsigned q = 0, qe = 0;
+  bool more = live;
+  while (__any_sync(0xffffffffu, more)) {
+    bool hit = false;
+    unsigned j = 0;
+    if (more) {
+      while (q >= qe) {
+        if (z > c1[2]) {
+          more = false;
+          break;
+        }
+        const size_t row = ((size_t)z * cg.g.dim[1] + y) * cg.g.dim[0];
+        q = start[row + c0[0]];
+        qe = start[row + c1[0] + 1];
+        if (++y > c1[1]) {
+          y = c0[1];
+          ++z;
+        }
+      }
+      if (more) {
+        j = order[q++];
+        hit = aabb_overlap(mine, bb + 6 * (size_t)j);
+      }
+    }
+    append_pair(hit, i, j + second_base, first, second, capacity, n_pairs);
+  }
+  const unsigned nover = counters[0];
+  for (unsigned k = 0; k < nover; ++k) {
+    const unsigned u = order[nb - 1u - k];
+    append_pair(live && aabb_overlap(mine, bb + 6 * (size_t)u), i, u + second_base, first, second, capacity, n_pairs);
+  }
+}
+// the A objects listed in `brute` against every B object: thread per B object j, loop over the (few) listed ones
+__global__ void __launch_bounds__(128) k_cross_brute(const double* ba, const double* bb, unsigned nb, const unsigned* counters,
+                                                     const unsigned* brute, uint32_t* first, uint32_t* second,
+                                                     unsigned second_base, unsigned capacity, unsigned* n_pairs) {
+  const unsigned nbr = counters[1];
+  if (nbr == 0) return;
+  const unsigned jend = (nb + 31u) & ~31u;  // (warp-uniform trip count for the ballots)
+  for (unsigned j = blockIdx.x * blockDim.x + threadIdx.x; j < jend; j += gridDim.x * blockDim.x) {
+    const bool jl = j < nb && !aabb_empty(bb + 6 * (size_t)j);
+    double mine[6] = {0, 0, 0, 0, 0, 0};
+    if (jl)
+      for (int k = 0; k < 6; ++k) mine[k] = bb[6 * (size_t)j + k];
+    for (unsigned q = 0; q < nbr; ++q) {
+      const unsigned a = brute[q];
+      append_pair(jl && aabb_overlap(ba + 6 * (size_t)a, mine), a, j + second_base, first, second, capacity, n_pairs);
+    }
+  }
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -306,7 +429,7 @@ int bp_pairs_launch(size_t n, const double* d_aabbs, size_t i_lo, size_t i_hi, u
   // the number of cells is only known on the device: counters are cleared and scanned for the maximum
   if ((e = cudaMemsetAsync(w.count, 0, (size_t)(kMaxCells + 1) * 4, s)) != cudaSuccess) return (int)e;
   if ((e = cudaMemsetAsync(w.cursor, 0, (size_t)kMaxCells * 4, s)) != cudaSuccess) return (int)e;
-  k_cell_hist<<<(nn + 255) / 256, 256, 0, s>>>(d_aabbs, nn, w.grid, w.cell, w.count, w.order, w.n_unbounded);
+  k_cell_hist<<<(nn + 255) / 256, 256, 0, s>>>(d_aabbs, nn, w.grid, w.cell, w.count, w.order, w.n_unbounded, nullptr);
   size_t tb = w.cub_bytes;
   if ((e = cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, w.count, w.start, (int)(kMaxCells + 1), s)) != cudaSuccess) return (int)e;
   k_cell_scatter<<<(nn + 255) / 256, 256, 0, s>>>(w.cell, nn, w.start, w.cursor, w.order);
@@ -322,6 +445,49 @@ int bp_pairs_launch(size_t n, const double* d_aabbs, size_t i_lo, size_t i_hi, u
     k_sweep_unbounded<<<ub ? ub : 1u, 128, 0, s>>>(d_aabbs, nn, (unsigned)i_lo, (unsigned)i_hi, w.cell, w.order, w.n_unbounded, d_first,
                                                    d_second, (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity), d_n_pairs);
   }
+  *launches += 5;
+  return (int)cudaGetLastError();
+}
+
+// the self form's scratch for B, then the extent histogram and the list of A objects tested against all of B
+size_t bp_cross_scratch_bytes(size_t n_a, size_t n_b) {
+  return bp_scratch_bytes(n_b) + up256((size_t)kExtBins * 4) + up256(n_a * 4);
+}
+
+int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
+                          uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity, unsigned* d_n_pairs,
+                          void* scratch, int num_sms, cudaStream_t s, int* launches) {
+  if (num_sms < 1) num_sms = 1;
+  Scratch w = carve(scratch, n_b);
+  unsigned char* extra = static_cast<unsigned char*>(scratch) + bp_scratch_bytes(n_b);
+  unsigned* hist = reinterpret_cast<unsigned*>(extra);
+  unsigned* brute = reinterpret_cast<unsigned*>(extra + up256((size_t)kExtBins * 4));
+  CrossGrid* cg = reinterpret_cast<CrossGrid*>(w.grid);  // (the grid slot has 256 bytes)
+  unsigned* counters = w.n_unbounded;                    // [0]: B oversize + unbounded, [1]: A brute
+  const unsigned nb = (unsigned)n_b;
+  const unsigned cap = (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity);
+  unsigned pb = (nb + 255) / 256;
+  if (pb > kParts) pb = kParts;
+  if (pb == 0) pb = 1;
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(hist, 0, (size_t)kExtBins * 4, s)) != cudaSuccess) return (int)e;
+  k_cross_bounds_partial<<<pb, 256, 0, s>>>(d_aabbs_b, nb, w.part, hist);
+  k_cross_grid<<<1, 256, 0, s>>>(w.part, pb, hist, cg, d_n_pairs, counters);
+  *launches += 2;
+  if (a_hi > n_a) a_hi = n_a;
+  if (n_b == 0 || a_lo >= a_hi) return (int)cudaGetLastError();
+  if ((e = cudaMemsetAsync(w.count, 0, (size_t)(kMaxCells + 1) * 4, s)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemsetAsync(w.cursor, 0, (size_t)kMaxCells * 4, s)) != cudaSuccess) return (int)e;
+  k_cell_hist<<<(nb + 255) / 256, 256, 0, s>>>(d_aabbs_b, nb, &cg->g, w.cell, w.count, w.order, counters, &cg->cell);
+  size_t tb = w.cub_bytes;
+  if ((e = cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, w.count, w.start, (int)(kMaxCells + 1), s)) != cudaSuccess) return (int)e;
+  k_cell_scatter<<<(nb + 255) / 256, 256, 0, s>>>(w.cell, nb, w.start, w.cursor, w.order);
+  k_cross_sweep<<<(unsigned)((a_hi - a_lo + 127) / 128), 128, 0, s>>>(d_aabbs_a, (unsigned)a_lo, (unsigned)a_hi, d_aabbs_b, nb, cg,
+                                                                      w.start, w.order, counters, brute, d_first, d_second,
+                                                                      second_base, cap, d_n_pairs);
+  unsigned ub = (nb + 127) / 128;
+  if (ub > (unsigned)num_sms * 8u) ub = (unsigned)num_sms * 8u;
+  k_cross_brute<<<ub, 128, 0, s>>>(d_aabbs_a, d_aabbs_b, nb, counters, brute, d_first, d_second, second_base, cap, d_n_pairs);
   *launches += 5;
   return (int)cudaGetLastError();
 }

@@ -173,14 +173,35 @@ struct BroadGrid {
   int dim[3];
 };
 HFB_HD int grid_coord(const BroadGrid& g, double c, int k) {
-  int v = (int)floor((c - g.origin[k]) * g.inv_cell);
-  return v < 0 ? 0 : (v >= g.dim[k] ? g.dim[k] - 1 : v);
+  // clamped before the conversion: a query box of the cross form may lie far outside the grid
+  const double v = floor((c - g.origin[k]) * g.inv_cell);
+  return !(v >= 0) ? 0 : (v >= g.dim[k] ? g.dim[k] - 1 : (int)v);
 }
 HFB_HD unsigned grid_cell(const BroadGrid& g, const double* bb) {
   const int x = grid_coord(g, 0.5 * (bb[0] + bb[3]), 0), y = grid_coord(g, 0.5 * (bb[1] + bb[4]), 1),
             z = grid_coord(g, 0.5 * (bb[2] + bb[5]), 2);
   return (unsigned)((z * g.dim[1] + y) * g.dim[0] + x);
 }
+// the grid over the centres' box [lo, hi] with cells of at least `cell`, grown until it has at most 2^21 cells;
+// returns the cell size used
+HFB_HD double grid_fit(const double* lo, const double* hi, double cell, BroadGrid& g) {
+  double dim[3];
+  for (;;) {
+    // counted in double: a cell far below the span must grow, not wrap the int dimensions
+    double cells = 1;
+    for (int k = 0; k < 3; ++k) {
+      dim[k] = floor((hi[k] - lo[k]) / cell) + 1;
+      cells *= dim[k];
+    }
+    if (cells <= 2097152.0) break;
+    cell *= 1.26;  // halves the number of cells
+  }
+  for (int k = 0; k < 3; ++k) g.dim[k] = (int)dim[k];
+  for (int k = 0; k < 3; ++k) g.origin[k] = lo[k];
+  g.inv_cell = 1.0 / cell;
+  return cell;
+}
+
 // a grid for these boxes: cell = the largest box extent (so partners sit in adjacent cells), at most ~2^21 cells
 inline BroadGrid make_grid(size_t n, const double* bb) {
   BroadGrid g;
@@ -195,18 +216,7 @@ inline BroadGrid make_grid(size_t n, const double* bb) {
     }
   }
   if (!(lo[0] <= hi[0])) lo[0] = lo[1] = lo[2] = hi[0] = hi[1] = hi[2] = 0;  // nothing bounded
-  double cell = ext > 0 ? ext : 1.0;
-  for (;;) {
-    double cells = 1;
-    for (int k = 0; k < 3; ++k) {
-      g.dim[k] = (int)floor((hi[k] - lo[k]) / cell) + 1;
-      cells *= g.dim[k];
-    }
-    if (cells <= 2097152.0) break;
-    cell *= 1.26;  // halves the number of cells
-  }
-  for (int k = 0; k < 3; ++k) g.origin[k] = lo[k];
-  g.inv_cell = 1.0 / cell;
+  grid_fit(lo, hi, ext > 0 ? ext : 1.0, g);
   return g;
 }
 
@@ -269,6 +279,139 @@ inline size_t broadphase_pairs_host(size_t n, const double* bb, uint32_t* first,
           }
         }
   }
+  return count;
+}
+
+// ---- cross form: every (i in A, j in B) with overlapping boxes --------------------------------------------------
+// BroadPhaseCollisionManager::collide(other, callback) (broadphase_collision_manager.h:94-118; the set of
+// NaiveCollisionManager::collide(other), src/broadphase/broadphase_bruteforce.cpp:150-170).  The grid is built over B
+// only, so the sizes of A's boxes never shape it.  Its cell is not B's largest extent (one wall among small objects
+// would put the whole environment in a handful of cells) but the power of two at or above the extents of 95 % of
+// B's bounded boxes (a log2 histogram of the extents).  B boxes wider than the final cell ("oversize") stay out of the
+// grid with B's unbounded ones and are tested against every A object.  A B box in the grid has its centre within
+// half a cell of any box it overlaps, so an A box looks up the cells its box covers widened by half a cell; the cells
+// of one grid row are contiguous in the sorted order, so a lookup walks one index range per row.  A boxes that are
+// unbounded or whose lookup spans more than kCrossScanRows rows are tested against every B object instead.  The
+// pairs are partitioned by (A grid / A brute) x (B grid / B oversize), so each is reported once.
+constexpr int kExtBins = 128;
+constexpr int kCrossScanRows = 256;
+
+HFB_HD double box_extent(const double* b) {
+  double e = b[3] - b[0];
+  e = b[4] - b[1] > e ? b[4] - b[1] : e;
+  return b[5] - b[2] > e ? b[5] - b[2] : e;
+}
+// histogram bin of an extent: bin b >= 1 holds [2^(b-64), 2^(b-63)), bin 0 the empty extents
+HFB_HD int extent_bin(double e) {
+  if (!(e > 0)) return 0;
+  const int b = ilogb(e) + 64;
+  return b < 1 ? 1 : (b >= kExtBins ? kExtBins - 1 : b);
+}
+// the cell the cross form starts from: the top of the bin that holds the 95th percentile of the extents.  Boxes of
+// zero extent (points) fit any cell: when they make up the percentile, the first non-empty bin above them sets the
+// cell, and with nothing but points the self form's fallback of 1 does
+HFB_HD double cross_cell(const unsigned* hist, unsigned total) {
+  if (total == 0) return 1.0;
+  const unsigned want = total - total / 20u;
+  unsigned cum = 0;
+  int b = 0;
+  for (; b < kExtBins - 1; ++b) {
+    cum += hist[b];
+    if (cum >= want) break;
+  }
+  if (b == 0)
+    for (b = 1; b < kExtBins && hist[b] == 0; ++b) {
+    }
+  return b < kExtBins ? ldexp(1.0, b - 63) : 1.0;
+}
+// B's grid over its centres' box [lo, hi]: the cell from the histogram, no finer than the largest span / 2^21 (a
+// finer one has more than 2^21 cells along that axis alone, so grid_fit would only grow it step by step)
+HFB_HD double cross_grid_fit(const double* lo, const double* hi, const unsigned* hist, unsigned total, BroadGrid& g) {
+  double cell = cross_cell(hist, total), span = 0;
+  for (int k = 0; k < 3; ++k) span = hi[k] - lo[k] > span ? hi[k] - lo[k] : span;
+  cell = cell > span * 0x1p-21 ? cell : span * 0x1p-21;
+  return grid_fit(lo, hi, cell, g);
+}
+// the grid cells an A box looks up: its box widened by half a cell, plus a margin that covers the rounding of the
+// centres (the grid coordinate is monotonic in the position, so a margin is all it takes)
+HFB_HD int cross_query_cells(const BroadGrid& g, double cell, const double* a, int* c0, int* c1) {
+  for (int k = 0; k < 3; ++k) {
+    const double m = 0.5 * cell * (1.0 + 1e-6) + 1e-12 * fmax(fabs(a[k]), fabs(a[3 + k]));
+    c0[k] = grid_coord(g, a[k] - m, k);
+    c1[k] = grid_coord(g, a[3 + k] + m, k);
+  }
+  return (c1[1] - c0[1] + 1) * (c1[2] - c0[2] + 1);  // rows
+}
+
+// the cross set in no particular order, (index in A, index in B); returns its size (all pairs are counted, at most
+// `capacity` stored)
+inline size_t broadphase_cross_pairs_host(size_t na, const double* ba, size_t nb, const double* bb, uint32_t* first,
+                                          uint32_t* second, size_t capacity) {
+  if (na == 0 || nb == 0) return 0;
+  double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+  unsigned hist[kExtBins] = {0}, total = 0;
+  for (size_t j = 0; j < nb; ++j) {
+    const double* b = bb + 6 * j;
+    if (aabb_empty(b) || aabb_unbounded(b)) continue;
+    for (int k = 0; k < 3; ++k) {
+      const double c = 0.5 * (b[k] + b[3 + k]);
+      lo[k] = c < lo[k] ? c : lo[k];
+      hi[k] = c > hi[k] ? c : hi[k];
+    }
+    ++hist[extent_bin(box_extent(b))];
+    ++total;
+  }
+  if (!(lo[0] <= hi[0])) lo[0] = lo[1] = lo[2] = hi[0] = hi[1] = hi[2] = 0;
+  BroadGrid g;
+  const double cell = cross_grid_fit(lo, hi, hist, total, g);
+  const size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
+  std::vector<uint32_t> cell_of(nb), start(ncell + 1, 0), order(nb), over, brute;
+  for (size_t j = 0; j < nb; ++j) {
+    const double* b = bb + 6 * j;
+    if (aabb_empty(b)) {
+      cell_of[j] = 0xffffffffu;
+    } else if (aabb_unbounded(b) || box_extent(b) > cell) {
+      cell_of[j] = 0xfffffffeu;
+      over.push_back((uint32_t)j);
+    } else {
+      cell_of[j] = grid_cell(g, b);
+      ++start[cell_of[j] + 1];
+    }
+  }
+  for (size_t c = 0; c < ncell; ++c) start[c + 1] += start[c];
+  {
+    std::vector<uint32_t> cur(start.begin(), start.end() - 1);
+    for (size_t j = 0; j < nb; ++j)
+      if (cell_of[j] < 0xfffffffeu) order[cur[cell_of[j]]++] = (uint32_t)j;
+  }
+  size_t count = 0;
+  auto emit = [&](size_t i, uint32_t j) {
+    if (count < capacity) {
+      first[count] = (uint32_t)i;
+      second[count] = j;
+    }
+    ++count;
+  };
+  for (size_t i = 0; i < na; ++i) {
+    const double* a = ba + 6 * i;
+    if (aabb_empty(a)) continue;
+    int c0[3], c1[3];
+    if (aabb_unbounded(a) || cross_query_cells(g, cell, a, c0, c1) > kCrossScanRows) {
+      brute.push_back((uint32_t)i);
+      continue;
+    }
+    for (int z = c0[2]; z <= c1[2]; ++z)
+      for (int y = c0[1]; y <= c1[1]; ++y) {
+        const size_t row = ((size_t)z * g.dim[1] + y) * g.dim[0];
+        for (uint32_t q = start[row + c0[0]]; q < start[row + c1[0] + 1]; ++q)
+          if (aabb_overlap(a, bb + 6 * (size_t)order[q])) emit(i, order[q]);
+      }
+    for (uint32_t j : over)
+      if (aabb_overlap(a, bb + 6 * (size_t)j)) emit(i, j);
+  }
+  for (uint32_t i : brute)
+    for (size_t j = 0; j < nb; ++j)
+      if (cell_of[j] != 0xffffffffu && aabb_overlap(ba + 6 * (size_t)i, bb + 6 * j)) emit(i, (uint32_t)j);
   return count;
 }
 

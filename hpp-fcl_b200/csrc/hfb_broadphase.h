@@ -19,5 +19,13 @@ size_t bp_scratch_bytes(size_t n);
 // launched.
 int bp_pairs_launch(size_t n, const double* d_aabbs, size_t i_lo, size_t i_hi, uint32_t* d_first, uint32_t* d_second,
                     size_t capacity, unsigned* d_n_pairs, void* scratch, int num_sms, cudaStream_t s, int* launches);
+// scratch the cross pair finder needs for n_a objects in A and n_b in B
+size_t bp_cross_scratch_bytes(size_t n_a, size_t n_b);
+// every (i, j), i in A with i in [a_lo, a_hi), j in B, with overlapping boxes -> (i, second_base + j), at most
+// `capacity` stored, all counted in *d_n_pairs (grid over B only: hfb_broadphase.cuh, broadphase_cross_pairs_host);
+// `scratch`: bp_cross_scratch_bytes(n_a, n_b) bytes.  Returns a cudaError_t as int; *launches += kernels launched.
+int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
+                          uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity, unsigned* d_n_pairs,
+                          void* scratch, int num_sms, cudaStream_t s, int* launches);
 
 }  // namespace hfb

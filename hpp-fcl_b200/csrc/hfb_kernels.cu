@@ -2415,34 +2415,18 @@ int hfb_broadphase_pairs_device(hfb_ctx* ctx, size_t n, const double* d_aabbs, s
   return HFB_OK;
 }
 
-// Broadphase + narrow phase of a scene in one call, everything on the device between the upload of the poses and the
-// download of the colliding pairs: the batched form of BroadPhaseCollisionManager::collide(callback) with the default
-// collision callback (broadphase/default_broadphase_callbacks.h:69-130: collide() of every candidate pair, contacts
-// collected).
-int hfb_scene_collide(hfb_ctx* ctx, size_t n, const uint32_t* handles, const hfb_transform* tfs, size_t first_object,
-                      size_t num_first_objects, const hfb_collision_request* req, const hfb_scene_contacts* out) {
-  if (!ctx || !req || !out || (n && (!handles || !tfs))) return HFB_ERR_INVALID_ARGUMENT;
-  if (out->capacity && (!out->first || !out->second || !out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
-  std::unique_lock<std::mutex> lk(ctx->mu);
-  bool minus_inf;
-  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
-  if (int rc = check_ready(ctx)) return rc;
-  if (n > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = check_handles(ctx, handles, n)) return rc;
-  if (out->n_candidates) *out->n_candidates = 0;
-  if (out->n_colliding) *out->n_colliding = 0;
-  if (n < 2) return HFB_OK;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->slots[0].stream;
-  CK(ctx->obj_h.reserve(n * 4 + 4));
-  CK(ctx->obj_tf.reserve(n * sizeof(hfb_transform) + 8));
+}  // extern "C"
+
+// The part hfb_scene_collide and hfb_scene_collide_sets share, after the upload of the object table (d_h, d_tf: n
+// objects): the boxes, the candidates (find_pairs(d_bb, pf, ps, capacity, d_count, &launches) launches a pair finder,
+// all pairs counted in *d_count, at most `capacity` stored), collide() of every candidate over the table, compaction
+// and download; `second_base` is subtracted from the downloaded second indices.
+template <class FindPairs>
+static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
+                               FindPairs find_pairs, uint32_t second_base, const hfb_collision_request* req, bool minus_inf,
+                               const hfb_scene_contacts* out) {
   CK(ctx->sc_bb.reserve(n * 48));
   CK(ctx->sc_cnt.reserve(16));
-  CK(ctx->bp_scratch.reserve(bp_scratch_bytes(n)));
-  CK(cudaMemcpyAsync(ctx->obj_h.p, handles, n * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(ctx->obj_tf.p, tfs, n * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
-  const uint32_t* d_h = static_cast<const uint32_t*>(ctx->obj_h.p);
-  const hfb_transform* d_tf = static_cast<const hfb_transform*>(ctx->obj_tf.p);
   double* d_bb = static_cast<double*>(ctx->sc_bb.p);
   unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
   if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n, d_h, d_tf, d_bb, s) != 0)
@@ -2450,13 +2434,11 @@ int hfb_scene_collide(hfb_ctx* ctx, size_t n, const uint32_t* handles, const hfb
   ctx->stats.kernel_launches++;
   // the number of candidate pairs is not known in advance: a first sweep counts, a second one (if the buffers were too
   // small) stores
-  const size_t i_hi = first_object + (num_first_objects < n ? num_first_objects : n);
-  size_t cap = ctx->sc_pf.cap / 4;
+  size_t cap = ctx->sc_pf.cap / 4 < ctx->sc_ps.cap / 4 ? ctx->sc_pf.cap / 4 : ctx->sc_ps.cap / 4;
   unsigned cand = 0;
   for (int attempt = 0; attempt < 2; ++attempt) {
     int nl = 0;
-    if (bp_pairs_launch(n, d_bb, first_object, i_hi, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p),
-                        cap, d_cnt, ctx->bp_scratch.p, ctx->num_sms, s, &nl) != 0)
+    if (find_pairs(d_bb, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p), cap, d_cnt, &nl) != 0)
       return fail(ctx, HFB_ERR_CUDA, "broadphase launch failed");
     ctx->stats.kernel_launches += (uint64_t)nl;
     CK(cudaMemcpyAsync(&cand, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
@@ -2500,8 +2482,113 @@ int hfb_scene_collide(hfb_ctx* ctx, size_t n, const uint32_t* handles, const hfb
     CK(cudaMemcpyAsync(out->second, ctx->sc_s.p, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(out->contacts, ctx->sc_rec.p, (size_t)kept * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
+    if (second_base)
+      for (unsigned k = 0; k < kept; ++k) out->second[k] -= second_base;
   }
   return HFB_OK;
+}
+
+extern "C" {
+
+// Broadphase + narrow phase of a scene in one call, everything on the device between the upload of the poses and the
+// download of the colliding pairs: the batched form of BroadPhaseCollisionManager::collide(callback) with the default
+// collision callback (broadphase/default_broadphase_callbacks.h:69-130: collide() of every candidate pair, contacts
+// collected).
+int hfb_scene_collide(hfb_ctx* ctx, size_t n, const uint32_t* handles, const hfb_transform* tfs, size_t first_object,
+                      size_t num_first_objects, const hfb_collision_request* req, const hfb_scene_contacts* out) {
+  if (!ctx || !req || !out || (n && (!handles || !tfs))) return HFB_ERR_INVALID_ARGUMENT;
+  if (out->capacity && (!out->first || !out->second || !out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
+  std::unique_lock<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = check_ready(ctx)) return rc;
+  if (n > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = check_handles(ctx, handles, n)) return rc;
+  if (out->n_candidates) *out->n_candidates = 0;
+  if (out->n_colliding) *out->n_colliding = 0;
+  if (n < 2) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  CK(ctx->obj_h.reserve(n * 4 + 4));
+  CK(ctx->obj_tf.reserve(n * sizeof(hfb_transform) + 8));
+  CK(ctx->bp_scratch.reserve(bp_scratch_bytes(n)));
+  CK(cudaMemcpyAsync(ctx->obj_h.p, handles, n * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->obj_tf.p, tfs, n * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  const size_t i_hi = first_object + (num_first_objects < n ? num_first_objects : n);
+  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+    return bp_pairs_launch(n, d_bb, first_object, i_hi, pf, ps, cap, d_cnt, ctx->bp_scratch.p, ctx->num_sms, s, nl);
+  };
+  return scene_collide_table(ctx, s, n, static_cast<const uint32_t*>(ctx->obj_h.p),
+                             static_cast<const hfb_transform*>(ctx->obj_tf.p), find, 0u, req, minus_inf, out);
+}
+
+// ---- broadphase between two sets: collide(other_manager, callback) / collide(obj, callback) --------------------
+// (broadphase/broadphase_collision_manager.h:94-118; grid over B only: hfb_broadphase.cuh)
+int hfb_broadphase_cross_pairs(size_t n_a, const double* aabbs_a, size_t n_b, const double* aabbs_b, uint32_t* first,
+                               uint32_t* second, size_t capacity, size_t* n_pairs) {
+  if ((n_a && !aabbs_a) || (n_b && !aabbs_b) || !n_pairs || (capacity && (!first || !second)) || n_a > 0xffffffffull ||
+      n_b > 0xffffffffull)
+    return HFB_ERR_INVALID_ARGUMENT;
+  *n_pairs = broadphase_cross_pairs_host(n_a, aabbs_a, n_b, aabbs_b, first, second, capacity);
+  return HFB_OK;
+}
+
+int hfb_broadphase_cross_pairs_device(hfb_ctx* ctx, size_t n_a, const double* d_aabbs_a, size_t first_a, size_t num_a,
+                                      size_t n_b, const double* d_aabbs_b, uint32_t* d_first, uint32_t* d_second,
+                                      size_t capacity, uint32_t* d_n_pairs, void* stream) {
+  if (!ctx || (n_a && !d_aabbs_a) || (n_b && !d_aabbs_b) || !d_n_pairs || (capacity && (!d_first || !d_second)) ||
+      n_a > 0xffffffffull || n_b > 0xffffffffull)
+    return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  CK(cudaSetDevice(ctx->device));
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  int nl = 0;
+  const size_t a_hi = first_a + (num_a < n_a ? num_a : n_a);
+  if (bp_cross_pairs_launch(n_a, d_aabbs_a, first_a, a_hi, n_b, d_aabbs_b, d_first, d_second, 0u, capacity, d_n_pairs,
+                            ctx->bp_scratch.p, ctx->num_sms, static_cast<cudaStream_t>(stream), &nl) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "cross broadphase launch failed");
+  ctx->stats.kernel_launches += (uint64_t)nl;
+  return HFB_OK;
+}
+
+// hfb_scene_collide for two sets: the object table on the device is [A; B], so the candidates are (i, n_a + j) there
+// and the narrow phase and the compaction are hfb_scene_collide's own; `second` is turned back into an index in B
+// after the download
+int hfb_scene_collide_sets(hfb_ctx* ctx, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a, size_t n_b,
+                           const uint32_t* handles_b, const hfb_transform* tfs_b, size_t first_a, size_t num_a,
+                           const hfb_collision_request* req, const hfb_scene_contacts* out) {
+  if (!ctx || !req || !out || (n_a && (!handles_a || !tfs_a)) || (n_b && (!handles_b || !tfs_b)))
+    return HFB_ERR_INVALID_ARGUMENT;
+  if (out->capacity && (!out->first || !out->second || !out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
+  std::unique_lock<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = check_ready(ctx)) return rc;
+  if (n_a > 0xffffffffull || n_b > 0xffffffffull || n_a + n_b > 0xffffffffull)
+    return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
+  if (int rc = check_handles(ctx, handles_b, n_b)) return rc;
+  if (out->n_candidates) *out->n_candidates = 0;
+  if (out->n_colliding) *out->n_colliding = 0;
+  if (n_a == 0 || n_b == 0) return HFB_OK;
+  const size_t n = n_a + n_b;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  CK(ctx->obj_h.reserve(n * 4 + 4));
+  CK(ctx->obj_tf.reserve(n * sizeof(hfb_transform) + 8));
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  uint32_t* d_h = static_cast<uint32_t*>(ctx->obj_h.p);
+  hfb_transform* d_tf = static_cast<hfb_transform*>(ctx->obj_tf.p);
+  CK(cudaMemcpyAsync(d_h, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_h + n_a, handles_b, n_b * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_tf, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(d_tf + n_a, tfs_b, n_b * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  const size_t a_hi = first_a + (num_a < n_a ? num_a : n_a);
+  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+    return bp_cross_pairs_launch(n_a, d_bb, first_a, a_hi, n_b, d_bb + 6 * n_a, pf, ps, (uint32_t)n_a, cap, d_cnt,
+                                 ctx->bp_scratch.p, ctx->num_sms, s, nl);
+  };
+  return scene_collide_table(ctx, s, n, d_h, d_tf, find, (uint32_t)n_a, req, minus_inf, out);
 }
 
 int hfb_batch_convex_support_device(hfb_ctx* ctx, size_t n, const uint32_t* ids, const double* dirs,

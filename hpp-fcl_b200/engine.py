@@ -63,6 +63,9 @@ def load_library(path=None):
     L.hfb_scene_aabbs_device.argtypes = [vp, sz, vp, vp, vp, vp]
     L.hfb_broadphase_pairs_device.argtypes = [vp, sz, vp, sz, sz, vp, vp, sz, vp, vp]
     L.hfb_scene_collide.argtypes = [vp, sz, vp, vp, sz, sz, vp, vp]
+    L.hfb_broadphase_cross_pairs.argtypes = [sz, vp, sz, vp, vp, vp, sz, vp]
+    L.hfb_broadphase_cross_pairs_device.argtypes = [vp, sz, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
+    L.hfb_scene_collide_sets.argtypes = [vp, sz, vp, vp, sz, vp, vp, sz, sz, vp, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -111,6 +114,27 @@ def broadphase_pairs(aabbs, capacity=None):
         rc = L.hfb_broadphase_pairs(n, _ptr(bb), _ptr(first), _ptr(second), cap, C.byref(cnt))
         if rc != 0:
             raise EngineError("hfb_broadphase_pairs: %s" % _ERR.get(rc, rc))
+        if cnt.value <= cap or capacity is not None:
+            k = min(cnt.value, cap)
+            return first[:k], second[:k]
+        cap = cnt.value
+
+
+def broadphase_cross_pairs(aabbs_a, aabbs_b, capacity=None):
+    """every (i, j), i a box of A, j a box of B (n x 6 each), whose boxes overlap, in no particular order -> (first =
+    index in A, second = index in B).  Host function of the library: needs neither a context nor a GPU."""
+    L = load_library()
+    ba = np.ascontiguousarray(aabbs_a, dtype=np.float64).reshape(-1, 6)
+    bb = np.ascontiguousarray(aabbs_b, dtype=np.float64).reshape(-1, 6)
+    cap = int(capacity) if capacity is not None else max(16 * (ba.shape[0] + bb.shape[0]), 1024)
+    while True:
+        first = np.empty(cap, dtype=np.uint32)
+        second = np.empty(cap, dtype=np.uint32)
+        cnt = C.c_size_t(0)
+        rc = L.hfb_broadphase_cross_pairs(ba.shape[0], _ptr(ba), bb.shape[0], _ptr(bb), _ptr(first), _ptr(second), cap,
+                                          C.byref(cnt))
+        if rc != 0:
+            raise EngineError("hfb_broadphase_cross_pairs: %s" % _ERR.get(rc, rc))
         if cnt.value <= cap or capacity is not None:
             k = min(cnt.value, cap)
             return first[:k], second[:k]
@@ -327,6 +351,37 @@ class Engine:
         out = P.SceneContacts(f.ctypes.data, s2.ctypes.data, rec.ctypes.data, cap, nc[0:1].ctypes.data, nc[1:2].ctypes.data)
         self._check(self.L.hfb_scene_collide(self.h, n, _ptr(oh), _ptr(ot), first_object,
                                              n if num_first_objects is None else num_first_objects, C.byref(req), C.byref(out)))
+        k = min(int(nc[0]), cap)
+        return f[:k], s2[:k], rec[:k], int(nc[1]), int(nc[0])
+
+    def broadphase_cross_pairs_device(self, n_a, d_aabbs_a, n_b, d_aabbs_b, d_first, d_second, capacity, d_n_pairs,
+                                      stream=0, first_a=0, num_a=None):
+        """pairs (i in A, j in B) with overlapping boxes, i in [first_a, first_a + num_a) (default: all of A)"""
+        self._check(self.L.hfb_broadphase_cross_pairs_device(self.h, n_a, _ptr(d_aabbs_a), first_a,
+                                                             n_a if num_a is None else num_a, n_b, _ptr(d_aabbs_b),
+                                                             _ptr(d_first), _ptr(d_second), capacity, _ptr(d_n_pairs),
+                                                             _ptr(stream)))
+
+    def scene_collide_sets(self, handles_a, tfs_a, handles_b, tfs_b, req=None, capacity=None, first_a=0, num_a=None,
+                           bufs=None):
+        """broadphase + narrow phase of set A against set B in one call (hfb_scene_collide_sets)
+        -> (first = index in A, second = index in B, contacts, n_candidates, n_colliding), in no particular order"""
+        req = req or P.CollisionRequestPOD()
+        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
+        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
+        hb = np.ascontiguousarray(handles_b, dtype=np.uint32)
+        tb = np.ascontiguousarray(tfs_b, dtype=P.transform_dtype)
+        if ha.shape[0] != ta.shape[0] or hb.shape[0] != tb.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        na, nb = ha.shape[0], hb.shape[0]
+        cap = int(capacity) if capacity is not None else max(4 * (na + nb), 1024)
+        if bufs is None:
+            bufs = (np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=P.contact_dtype))
+        f, s2, rec = bufs
+        nc = np.zeros(2, dtype=np.uint32)
+        out = P.SceneContacts(f.ctypes.data, s2.ctypes.data, rec.ctypes.data, cap, nc[0:1].ctypes.data, nc[1:2].ctypes.data)
+        self._check(self.L.hfb_scene_collide_sets(self.h, na, _ptr(ha), _ptr(ta), nb, _ptr(hb), _ptr(tb), first_a,
+                                                  na if num_a is None else num_a, C.byref(req), C.byref(out)))
         k = min(int(nc[0]), cap)
         return f[:k], s2[:k], rec[:k], int(nc[1]), int(nc[0])
 

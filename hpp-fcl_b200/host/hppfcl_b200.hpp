@@ -752,12 +752,61 @@ class DynamicAABBTreeCollisionManager {
     first.resize(cnt);
     second.resize(cnt);
   }
+  /// every object of this manager against every object of `other`: callback(o1 from this manager, o2 from other)
+  /// for every pair with overlapping boxes until it returns true (broadphase_collision_manager.h:110-118);
+  /// collide(this, callback) is the self form
+  void collide(DynamicAABBTreeCollisionManager* other, CollisionCallBackBase* callback) {
+    if (other == this) return collide(callback);
+    callback->init();
+    std::vector<uint32_t> first, second;
+    pairs(*other, first, second);
+    for (size_t k = 0; k < first.size(); ++k)
+      if ((*callback)(objs[first[k]], other->objs[second[k]])) return;
+  }
+  /// one object against every object of this manager: callback(the manager's object, obj), the order of
+  /// DynamicAABBTreeCollisionManager::collide(obj, callback) (broadphase_dynamic_AABB_tree.cpp:361-390; the naive
+  /// manager passes (obj, object) instead).  obj's box is computed here, as setup() computes the manager's.
+  void collide(CollisionObject* obj, CollisionCallBackBase* callback) {
+    callback->init();
+    if (stale) refresh();
+    const uint32_t h = C.handle(obj->collisionGeometryPtr());
+    C.commit();
+    const hfb_transform t = obj->getTransform().pod();
+    double bb[6];
+    C.check(hfb_scene_aabbs(C.raw(), 1, &h, &t, bb));
+    obj->getAABB().min_ = Vec3f(bb[0], bb[1], bb[2]);
+    obj->getAABB().max_ = Vec3f(bb[3], bb[4], bb[5]);
+    std::vector<uint32_t> first, second;
+    cross_pairs(bb, 1, first, second);
+    for (size_t k = 0; k < first.size(); ++k)
+      if ((*callback)(objs[first[k]], obj)) return;
+  }
+  /// the cross candidates as object indices: first in this manager, second in `other`; pairs(*this, ...) is the self
+  /// form (first < second), as collide(this, callback) is
+  void pairs(DynamicAABBTreeCollisionManager& other, std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
+    if (&other == this) return pairs(first, second);
+    if (stale) refresh();
+    if (other.stale) other.refresh();
+    cross_pairs(other.boxes.data(), other.objs.size(), first, second);
+  }
   /// the object table of the scene in the form hfb_batch_*_objects takes
   const std::vector<uint32_t>& handles() const { return hs; }
   const std::vector<hfb_transform>& transforms() const { return tfs; }
   Context& context() { return C; }
 
  private:
+  void cross_pairs(const double* boxes_b, size_t n_b, std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
+    size_t cap = std::max<size_t>(16 * (objs.size() + n_b), 1024), cnt = 0;
+    for (;;) {
+      first.resize(cap);
+      second.resize(cap);
+      C.check(hfb_broadphase_cross_pairs(objs.size(), boxes.data(), n_b, boxes_b, first.data(), second.data(), cap, &cnt));
+      if (cnt <= cap) break;
+      cap = cnt;
+    }
+    first.resize(cnt);
+    second.resize(cnt);
+  }
   void refresh() {
     hs.resize(objs.size());
     tfs.resize(objs.size());
@@ -799,6 +848,36 @@ inline std::vector<hfb_contact> collide(DynamicAABBTreeCollisionManager& manager
   sc.n_pairs = first.size();
   sc.first = first.data();
   sc.second = second.data();
+  std::vector<hfb_contact> out(first.size());
+  manager.context().check(hfb_batch_collide_objects(manager.context().raw(), &sc, &q, out.data(), nullptr, nullptr));
+  return out;
+}
+
+/// the cross form in one call: the candidates of manager x other (first: index in `manager`, second: index in `other`)
+/// through the batched narrow phase over the object table [manager; other], o1 from `manager`.  Returns, per
+/// candidate pair, the record hfb_batch_collide writes.  collide(m, m, ...) is the self form collide(m, ...).
+inline std::vector<hfb_contact> collide(DynamicAABBTreeCollisionManager& manager, DynamicAABBTreeCollisionManager& other,
+                                        const CollisionRequest& request, std::vector<uint32_t>& first,
+                                        std::vector<uint32_t>& second) {
+  if (&other == &manager) return collide(manager, request, first, second);
+  if (request.num_max_contacts == 0 && request.security_margin != -std::numeric_limits<FCL_REAL>::infinity())
+    throw std::invalid_argument("Invalid number of max contacts (current value is 0).");
+  manager.pairs(other, first, second);
+  hfb_collision_request q;
+  detail::fill(request, q);
+  std::vector<uint32_t> hs(manager.handles());
+  hs.insert(hs.end(), other.handles().begin(), other.handles().end());
+  std::vector<hfb_transform> tfs(manager.transforms());
+  tfs.insert(tfs.end(), other.transforms().begin(), other.transforms().end());
+  std::vector<uint32_t> table_second(second);
+  for (uint32_t& s : table_second) s += (uint32_t)manager.handles().size();
+  hfb_object_pairs sc;
+  sc.n_objects = hs.size();
+  sc.object_handles = hs.data();
+  sc.object_tfs = tfs.data();
+  sc.n_pairs = first.size();
+  sc.first = first.data();
+  sc.second = table_second.data();
   std::vector<hfb_contact> out(first.size());
   manager.context().check(hfb_batch_collide_objects(manager.context().raw(), &sc, &q, out.data(), nullptr, nullptr));
   return out;

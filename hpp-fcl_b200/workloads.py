@@ -241,3 +241,98 @@ def config5_moving_boxes(n_objects=100_000, env_scale=None, seed=0xFC1 + 5, targ
         return out
 
     return dict(shapes=shapes, obj_h=obj_h, obj_tf=tf, env_scale=env_scale, step=step)
+
+
+def _axis_rotations(axis, ang):
+    """rotations by `ang` (n,) about the unit axis x (0), y (1) or z (2) -> (n, 3, 3)"""
+    c, s = np.cos(ang), np.sin(ang)
+    R = np.zeros(ang.shape + (3, 3))
+    i, j = [(1, 2), (2, 0), (0, 1)][axis]
+    R[..., axis, axis] = 1
+    R[..., i, i] = c
+    R[..., j, j] = c
+    R[..., i, j] = -s
+    R[..., j, i] = s
+    return R
+
+
+def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, seed=0xFC1 + 6, target_pairs=1_000_000):
+    """A planner's collision query: a seeded chain robot of n_links links (capsules, boxes and two small hulls, joint
+    axes alternating z / y) at n_configs configurations (random base in the room, random joint angles) -- set A,
+    n_configs * n_links objects, configuration-major -- against a static environment -- set B: small primitives
+    (spheres, boxes, capsules, cylinders of 2-8 cm), about 1 % large boxes (tables, shelves: 0.4-1.2 m), a few OBBRSS
+    meshes and a Halfspace floor z <= 0.  `room` (side of the square room, 1.7 m high) defaults to the value that gives
+    about `target_pairs` candidate pairs.
+    -> dict: link_len; geometry to register (`register(scene, oracle=False)` -> one handle per geometry slot);
+    geom_a / geom_b (geometry slot of every object) and tf_a / tf_b (poses)."""
+    rng = np.random.default_rng(seed)
+    link_len = 0.22
+    # robot geometry: slot k = link k; links 5 and 11 are hulls, every third of the others a box, the rest capsules
+    hull_links = (5, 11)
+    link_rec = []
+    for k in range(n_links):
+        if k % 3 == 2 and k not in hull_links:
+            link_rec.append((P.GEOM_BOX, [0.04, 0.04, 0.5 * link_len]))
+        else:
+            link_rec.append((P.GEOM_CAPSULE, [0.035, 0.5 * link_len - 0.035, 0.0]))
+    hulls = [ellipsoid_hull(rng, 24, radii=(0.05, 0.05, 0.5 * link_len)) for _ in hull_links]
+    # environment pools: 64 small primitives, 16 large boxes, one mesh
+    small = random_primitive_shapes(rng, 64, (P.GEOM_SPHERE, P.GEOM_BOX, P.GEOM_CAPSULE, P.GEOM_CYLINDER))
+    small["p"] *= 0.04  # radii / half sides 2 mm - 4 cm, so boxes of 2-8 cm
+    big = P.make_shapes([P.GEOM_BOX] * 16, 0.2 + 0.4 * rng.random((16, 3)))
+    mesh = sphere_mesh(0.15, 16, 8, noise=0.02, rng=rng)
+    n_prims = n_links + len(small) + len(big)
+    prim_types = np.array([t for t, _ in link_rec], dtype=np.uint32)
+    prim_p = np.array([p for _, p in link_rec], dtype=np.float64)
+    shapes = np.concatenate([P.make_shapes(prim_types, prim_p), small, big])
+    slot_hull = [n_prims, n_prims + 1]
+    slot_mesh = n_prims + 2
+    slot_floor = n_prims + 3
+
+    def register(sc, oracle=False):
+        h = [np.asarray(sc.register_shapes(shapes), dtype=np.uint32)]
+        for pts, tris in hulls:
+            cid = sc.register_convex(pts, tris) if oracle else sc.register_convex(pts)
+            h.append(np.asarray(sc.register_shapes(P.make_shapes([P.GEOM_CONVEX], [[0, 0, 0]], data=[cid])), dtype=np.uint32))
+        if oracle:
+            bid = sc.register_bvh(*mesh)[0]
+        else:
+            from .engine import build_bvh_obbrss
+            bid = sc.register_bvh_obbrss(build_bvh_obbrss(*mesh), *mesh)
+        h.append(np.asarray(sc.register_shapes(P.make_shapes([P.BV_OBBRSS], [[0, 0, 0]], data=[bid])), dtype=np.uint32))
+        h.append(np.asarray(sc.register_halfspaces(P.GEOM_HALFSPACE, [[0, 0, 1, 0.0]]), dtype=np.uint32))
+        return np.concatenate(h)
+
+    if room is None:
+        # candidates per link ~ density * (link box + object box)^3, about 0.25^3 for this robot and the small objects
+        room = float(np.sqrt(n_env * n_configs * n_links * 0.0136 / (1.7 * target_pairs)))
+    # ---- set B: the environment
+    geom_b = np.empty(n_env, dtype=np.int64)
+    kind = rng.random(n_env)
+    n_mesh = 8
+    geom_b[:] = n_links + rng.integers(0, len(small), n_env)
+    nbig = kind < 0.01
+    geom_b[nbig] = n_links + len(small) + rng.integers(0, len(big), int(nbig.sum()))
+    geom_b[1:1 + n_mesh] = slot_mesh
+    geom_b[0] = slot_floor
+    tf_b = random_transforms(rng, n_env, (0, 0, 0), (room, room, 1.7))
+    tf_b[nbig] = identity_transforms(int(nbig.sum()), T=tf_b["T"][nbig])  # axis-aligned furniture
+    tf_b[0] = identity_transforms(1)[0]
+    # ---- set A: the robot at n_configs configurations
+    K, L = n_configs, n_links
+    base = rng.random((K, 3)) * np.array([room, room, 0.0])
+    R = _axis_rotations(2, 2 * np.pi * rng.random(K))
+    p = base.copy()
+    Rs, Ts = np.empty((K, L, 3, 3)), np.empty((K, L, 3))
+    for k in range(L):
+        R = R @ _axis_rotations(2 if k % 2 == 0 else 1, rng.uniform(-1.2, 1.2, K) if k else rng.uniform(0, 2 * np.pi, K))
+        axis = R[:, :, 2]
+        Rs[:, k] = R
+        Ts[:, k] = p + 0.5 * link_len * axis
+        p = p + link_len * axis
+    tf_a = P.make_transforms(Rs.reshape(-1, 3, 3), Ts.reshape(-1, 3))
+    geom_a = np.tile(np.where(np.isin(np.arange(L), hull_links), 0, np.arange(L)), K)
+    for s, k in zip(slot_hull, hull_links):
+        geom_a[np.arange(K) * L + k] = s
+    return dict(register=register, geom_a=geom_a, tf_a=tf_a, geom_b=geom_b, tf_b=tf_b, room=room, link_len=link_len,
+                n_configs=K, n_links=L)

@@ -414,6 +414,30 @@ int hfb_scene_collide(hfb_ctx* ctx, size_t n_objects, const uint32_t* object_han
                       size_t first_object, size_t num_first_objects, const hfb_collision_request* req,
                       const hfb_scene_contacts* out);
 
+/* ---- broadphase between two object sets: BroadPhaseCollisionManager::collide(other_manager, callback) and
+ * collide(obj, callback) (include/hpp/fcl/broadphase/broadphase_collision_manager.h:94-118) ----------------------
+ * The candidates are every (i, j), i in set A, j in set B, whose boxes overlap (AABB::overlap, closed intervals) --
+ * the set NaiveCollisionManager::collide(other) reports (src/broadphase/broadphase_bruteforce.cpp:150-170), with
+ * first = i (index in A) and second = j (index in B): o1 from the manager called, o2 from `other`.  Objects without a
+ * box take no part; halfspaces and planes take part with their unbounded boxes (DynamicAABBTreeCollisionManager's
+ * tighter halfspace leaf test, AABB::overlap(const Halfspace&), is not reproduced, as in the self form).  In no
+ * particular order; all counted in *n_pairs, at most `capacity` stored.
+ * hfb_broadphase_cross_pairs: HOST function, no context.  hfb_broadphase_cross_pairs_device: DEVICE buffers,
+ * asynchronous on `cuda_stream` (the count is a device word); only the A objects in [first_a, first_a + num_a) --
+ * one GPU's share of the configurations -- report their pairs. */
+int hfb_broadphase_cross_pairs(size_t n_a, const double* aabbs_a, size_t n_b, const double* aabbs_b, uint32_t* first,
+                               uint32_t* second, size_t capacity, size_t* n_pairs);
+int hfb_broadphase_cross_pairs_device(hfb_ctx* ctx, size_t n_a, const double* d_aabbs_a, size_t first_a, size_t num_a,
+                                      size_t n_b, const double* d_aabbs_b, uint32_t* d_first, uint32_t* d_second,
+                                      size_t capacity, uint32_t* d_n_pairs, void* cuda_stream);
+/* Broadphase and narrow phase of set A against set B in ONE call, as hfb_scene_collide does for one set: HOST buffers,
+ * blocking; boxes, cross pairs, collide() of every candidate (o1 from A, o2 from B, as hfb_batch_collide_objects over
+ * the table [A; B]) and compaction on the device.  out->first = index in A, out->second = index in B; candidates and
+ * colliding pairs are all counted.  [first_a, first_a + num_a) as in hfb_broadphase_cross_pairs_device. */
+int hfb_scene_collide_sets(hfb_ctx* ctx, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a, size_t n_b,
+                           const uint32_t* handles_b, const hfb_transform* tfs_b, size_t first_a, size_t num_a,
+                           const hfb_collision_request* req, const hfb_scene_contacts* out);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
