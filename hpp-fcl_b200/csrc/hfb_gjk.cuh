@@ -66,6 +66,14 @@ HFB_HD SV gjk_support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, i
   sv.w = sv.w0 - sv.w1;
   return sv;
 }
+// the same, with the pose and the shapes' parameters read from `mr` (see mink_support)
+template <int G, int CAPS, class Mink>
+HFB_HD SV gjk_support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, int& h0, int& h1, const Mink& mr) {
+  SV sv;
+  mink_support<G, CAPS>(a, b, md, d, sv.w0, sv.w1, h0, h1, mr);
+  sv.w = sv.w0 - sv.w1;
+  return sv;
+}
 
 // Where gjk_step appends a support point and the witness points read them back: InRegs keeps the whole SV in the
 // simplex (every caller but the GJK passes, which keep w0 / w1 in a per-thread store of their own, SlotStore in
@@ -74,10 +82,24 @@ HFB_HD SV gjk_support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, i
 // projections it calls, instead of calling them out of line (in a kernel held to few registers an out-of-line call
 // saves and restores registers in local memory).  The tetrahedron projection is always called out of line: GJK's
 // witness points never reach it (a rank-4 simplex encloses the origin, which is a collision), and inlined it would
-// add ~20 KB of code.
+// add ~20 KB of code.  support: GJK::getSupport with the pose and the shapes' parameters of the MinkD and the shape
+// records (the passes read them from their store); ssr, upper_bound: the sum of the radii and the early-stop bound
+// gjk_begin put in the loop state.
 struct InRegs {
   using V = SV;
   static constexpr bool inline_projections = false;
+  template <int G, int CAPS>
+  HFB_HD SV support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, int& h0, int& h1) const {
+    return gjk_support<G, CAPS>(a, b, md, d, h0, h1);
+  }
+  template <class Loop>
+  HFB_HD double ssr(const Loop& L) const {
+    return L.ssr;
+  }
+  template <class Loop>
+  HFB_HD double upper_bound(const Loop& L, const GjkParams&) const {
+    return L.upper_bound;
+  }
   HFB_HD v3 append(GjkState& g, const SV& nv) const {
     put(g, g.rank, nv);
     return nv.w;
@@ -355,8 +377,10 @@ HFB_HD void gjk_begin(const MinkD& md, const GjkParams& P, v3 guess, int hint0, 
 }
 
 // one pass through the body of the do-while; returns whether the loop goes on.  `st` appends the new support point
-// (InRegs, or the passes' SlotStore; its vertex type is the simplex's).
-template <int G, int CAPS, class Store = InRegs>
+// and gives the relative pose and the shapes' parameters to the support calls (InRegs, or the passes' SlotStore; its
+// vertex type is the simplex's).  MOMENTUM false: the caller guarantees L.variant is HFB_GJK_DEFAULT, so L.w and L.dir are written
+// before they are read in every step and are not live from one step to the next.
+template <int G, int CAPS, class Store = InRegs, bool MOMENTUM = true>
 HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const GjkParams& P,
                      GjkStateT<typename Store::V>& g, GjkLoop& L, const Store& st = Store()) {
   const double tol = P.tolerance;
@@ -367,7 +391,7 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
     return false;
   }
   // support direction (:246-278)
-  if (L.variant == HFB_GJK_DEFAULT) {
+  if (!MOMENTUM || L.variant == HFB_GJK_DEFAULT) {
     L.dir = g.ray;
   } else if (L.variant == HFB_GJK_NESTEROV) {
     if (md.normalize_support_direction) {
@@ -386,20 +410,20 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
   }
 
   // appendVertex(curr_simplex, -dir, support_hint) (:281)
-  const SV nv = gjk_support<G, CAPS>(sa, sb, md, -L.dir, g.hint0, g.hint1);
+  const SV nv = st.template support<G, CAPS>(sa, sb, md, -L.dir, g.hint0, g.hint1);
   L.w = st.append(g, nv);
   g.rank += 1;
 
   // check B (:288-293)
   const double omega = dot(L.dir, L.w) / nrm(L.dir);
-  if (omega > L.upper_bound) {
-    g.distance = omega - L.ssr;
+  if (omega > st.upper_bound(L, P)) {
+    g.distance = omega - st.ssr(L);
     g.status = HFB_GJK_NO_COLLISION_EARLY_STOPPED;
     return false;
   }
 
   // drop the momentum when the Frank-Wolfe duality gap closes (:296-304)
-  if (L.variant != HFB_GJK_DEFAULT) {
+  if (MOMENTUM && L.variant != HFB_GJK_DEFAULT) {
     const double fw_gap = 2 * dot(g.ray, g.ray - L.w);
     if (fw_gap - tol <= 0) {
       g.rank -= 1;  // removeVertex
@@ -412,11 +436,11 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
   const bool cv = gjk_converged(P, g.ray, L.w, L.rl, L.alpha, omega);
   if (g.iterations > 0 && cv) {
     g.rank -= 1;  // removeVertex
-    if (L.variant != HFB_GJK_DEFAULT) {
+    if (MOMENTUM && L.variant != HFB_GJK_DEFAULT) {
       L.variant = HFB_GJK_DEFAULT;
       return true;  // `continue`
     }
-    g.distance = L.rl - L.ssr;
+    g.distance = L.rl - st.ssr(L);
     g.status = (g.distance < tol) ? HFB_GJK_COLLISION_WITH_PENETRATION : HFB_GJK_NO_COLLISION;
     return false;
   }

@@ -20,21 +20,89 @@
 //
 // Inside k_gjk_first and k_gjk_more a simplex vertex is w and a slot id (SVSlot): the support points w0 / w1, which
 // the iterations never read, wait in a per-thread store in shared memory (SlotStore) until the pair's loop state is
-// saved, its witness points are summed (their weights come from w) or its EPA item is written.  That leaves
-// registers for 3 blocks of 128 threads per SM instead of 2.
+// saved, its witness points are summed (their weights come from w) or its EPA item is written.  What the iterations
+// read but never write (the relative pose, the shapes' parameters, the radii) waits there as well, and is read again
+// where it is needed.  That leaves registers for 4 blocks of 128 threads per SM in the first pass instead of 3.
 #include "hfb_gjkpass.h"
 
 namespace {
 
-enum { PASS_THREADS = 128, PASS_BLOCKS_PER_SM = 3 };  // k_gjk_first / k_gjk_more: block size, resident blocks per SM
+// k_gjk_first / k_gjk_more: block size, resident blocks per SM.  4 for the first pass of the default variant, which
+// every pair goes through and which gains from the extra warps.  3 for the later passes: they run the long pairs, a
+// few per SM, where the length of one iteration's dependent chain counts more than the warps that hide it, so they
+// keep the pose in registers rather than read it from shared memory in every iteration.  3 for the Polyak and
+// Nesterov variants as well: they carry L.w and L.dir from one iteration to the next, which does not fit the registers
+// of 4 blocks without spilling in the loop.
+enum { PASS_THREADS = 128, PASS_BLOCKS_PER_SM_FIRST = 4, PASS_BLOCKS_PER_SM = 3 };
+constexpr int pass_blocks_per_sm(bool first, bool momentum) {
+  return first && !momentum ? PASS_BLOCKS_PER_SM_FIRST : PASS_BLOCKS_PER_SM;
+}
 
 // w0 / w1 of the simplex vertices of the passes: 4 slots per thread, laid out [slot][component][thread] so that the
 // lanes of a warp touch consecutive doubles (24 KB per block).  gjk_step appends a support point in the lowest slot no
 // live vertex uses: at most 3 vertices are live when it appends, so one is always free.
+// Next to them, what a pair reads but never writes while it iterates: the two radii (finishing reads them) and, with
+// POSE, the relative pose oR1 / ot1 of its Minkowski difference and the parameters p0..p2 of both shapes (the support
+// calls read them), laid out [row][thread] (2 or 20 KB per block).  Without POSE (the passes that run 3 blocks per
+// SM) the support calls read the pose and the parameters from registers.
+enum { RADII_ROWS = 2, POSE_ROWS = 20 };  // ssr0, ssr1; then oR1 row-major (9), ot1 (3), p0..p2 of each shape
+template <bool POSE>
 struct SlotStore {
   using V = SVSlot;
-  static constexpr bool inline_projections = true;  // (168 registers per thread)
-  double* col;  // this thread's column: component c of slot j at col[(6 * j + c) * PASS_THREADS]
+  static constexpr bool inline_projections = true;
+  static constexpr int rows = POSE ? POSE_ROWS : RADII_ROWS;
+  double* col;   // this thread's column: component c of slot j at col[(6 * j + c) * PASS_THREADS]
+  double* pose;  // this thread's column of the `rows` rows: row c at pose[c * PASS_THREADS]
+
+  __device__ __forceinline__ void set_pose(const GjkSetup& S) const {
+    const MinkD& md = S.md;
+    const double v[POSE_ROWS] = {md.ssr0,     md.ssr1,     md.oR1.r0.x, md.oR1.r0.y, md.oR1.r0.z,
+                                 md.oR1.r1.x, md.oR1.r1.y, md.oR1.r1.z, md.oR1.r2.x, md.oR1.r2.y,
+                                 md.oR1.r2.z, md.ot1.x,    md.ot1.y,    md.ot1.z,    S.a.p0,
+                                 S.a.p1,      S.a.p2,      S.b.p0,      S.b.p1,      S.b.p2};
+#pragma unroll
+    for (int c = 0; c < rows; ++c) pose[c * PASS_THREADS] = v[c];
+  }
+  // row c (read through a volatile pointer: otherwise the compiler forwards what set_pose stored and keeps it in
+  // registers across the iterations)
+  __device__ __forceinline__ double pr(int c) const {
+    return static_cast<const volatile double*>(pose)[c * PASS_THREADS];
+  }
+  __device__ __forceinline__ double ssr0() const { return pr(0); }
+  __device__ __forceinline__ double ssr1() const { return pr(1); }
+  __device__ __forceinline__ m3 oR1() const {
+    m3 R;
+    R.r0 = mk(pr(2), pr(3), pr(4));
+    R.r1 = mk(pr(5), pr(6), pr(7));
+    R.r2 = mk(pr(8), pr(9), pr(10));
+    return R;
+  }
+  __device__ __forceinline__ v3 ot1() const { return mk(pr(11), pr(12), pr(13)); }
+  // what gjk_begin puts in L.ssr and L.upper_bound, with POSE computed again (same operations) rather than kept in
+  // registers
+  __device__ __forceinline__ double ssr(const GjkLoop& L) const {
+    if constexpr (POSE) return ssr0() + ssr1();
+    else return L.ssr;
+  }
+  __device__ __forceinline__ double upper_bound(const GjkLoop& L, const GjkParams& P) const {
+    if constexpr (POSE) return P.distance_upper_bound + ssr(L);
+    else return L.upper_bound;
+  }
+  __device__ __forceinline__ ShapeD shape_at(const ShapeD& s, int c) const {
+    ShapeD r = s;
+    r.p0 = pr(c);
+    r.p1 = pr(c + 1);
+    r.p2 = pr(c + 2);
+    return r;
+  }
+  __device__ __forceinline__ ShapeD shape0(const ShapeD& s) const { return shape_at(s, 14); }
+  __device__ __forceinline__ ShapeD shape1(const ShapeD& s) const { return shape_at(s, 17); }
+  template <int G, int CAPS>
+  __device__ __forceinline__ SV support(const ShapeD& a, const ShapeD& b, const MinkD& md, v3 d, int& h0,
+                                        int& h1) const {
+    if constexpr (POSE) return gjk_support<G, CAPS>(a, b, md, d, h0, h1, *this);
+    else return gjk_support<G, CAPS>(a, b, md, d, h0, h1);
+  }
 
   __device__ __forceinline__ void st(int j, v3 w0, v3 w1) const {
     double* p = col + 6 * j * PASS_THREADS;
@@ -102,8 +170,9 @@ __device__ __forceinline__ v3 ld3r(const double* d, size_t stride, int row, unsi
 
 // the loop state of a pair that goes on into the next pass.  L.w and L.dir are only carried from one iteration to
 // the next by the Polyak and Nesterov variants (gjk_step overwrites both before it reads them otherwise).
+template <class Store>
 __device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q, const GjkStateT<SVSlot>& g,
-                                             const GjkLoop& L, bool momentum, const SlotStore& ss) {
+                                             const GjkLoop& L, bool momentum, const Store& ss) {
   r.i[RI_RANK * m + q] = g.rank;
   r.i[RI_ITER * m + q] = (int)g.iterations;
   r.i[RI_HINT0 * m + q] = g.hint0;
@@ -129,8 +198,9 @@ __device__ __forceinline__ void save_running(const Rows& r, size_t m, unsigned q
 // the inverse of save_running; status and distance are those of gjk_begin (a running pair has no result yet), ssr
 // and upper_bound are recomputed as gjk_begin computes them.  Vertex j's support points go to store slot j; the
 // vertices at and above `rank` are left unset (the next support point is written there before anything reads them).
+template <bool MOM, class Store>
 __device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q, const MinkD& md, const GjkParams& P,
-                                             GjkStateT<SVSlot>& g, GjkLoop& L, const SlotStore& ss) {
+                                             GjkStateT<SVSlot>& g, GjkLoop& L, const Store& ss) {
   g.status = HFB_GJK_NO_COLLISION;
   g.distance = 0.0;
   g.rank = r.i[RI_RANK * m + q];
@@ -154,7 +224,7 @@ __device__ __forceinline__ void load_running(const Rows& r, size_t m, unsigned q
       put(g, j, v);
     }
   }
-  if (P.variant != HFB_GJK_DEFAULT) {
+  if (MOM) {
     L.variant = r.i[RI_VARIANT * m + q];
     L.w = ld3r(r.d, m, RD_LW, q);
     L.dir = ld3r(r.d, m, RD_DIR, q);
@@ -183,11 +253,10 @@ __device__ __forceinline__ PairOut begin_out(const BatchArgs& a, unsigned i) {
 
 // pair_gjk_end of a pair whose iterations ended: its EPA queue item, or its result record.  Of what make_setup<CAP_PRIM>
 // builds, the extractors read the first pose, `swapped` (false) and the two radii.  The radii are kept from the set-up
-// (reading them again costs two dependent loads, handle then shape record, on the pair's last step); the pose, which
-// the iterations do not need, is read again here rather than kept in registers.
-template <int MODE>
-__device__ __forceinline__ void finish_pair(const BatchArgs& a, unsigned i, GjkStateT<SVSlot>& g, const SlotStore& ss,
-                                            double ssr0, double ssr1) {
+// in the store (reading them again costs two dependent loads, handle then shape record, on the pair's last step); the
+// first pose, which the iterations do not need, is read again here.
+template <int MODE, class Store>
+__device__ __forceinline__ void finish_pair(const BatchArgs& a, unsigned i, GjkStateT<SVSlot>& g, const Store& ss) {
   if (g.status == HFB_GJK_COLLISION && a.P.compute_penetration) {  // the EPA case of pair_gjk_end
     push_epa_item(a, i, g, ss);
     return;
@@ -195,8 +264,8 @@ __device__ __forceinline__ void finish_pair(const BatchArgs& a, unsigned i, GjkS
   GjkSetup S;
   S.tfa = load_xf(a.tf1[i].R);
   S.swapped = false;
-  S.md.ssr0 = ssr0;
-  S.md.ssr1 = ssr1;
+  S.md.ssr0 = ss.ssr0();
+  S.md.ssr1 = ss.ssr1();
   PairOut o = begin_out(a, i);
   pair_gjk_end<true>(a.P, S, g, o, ss);
   store_result<MODE>(a, i, o);
@@ -215,18 +284,20 @@ __device__ __forceinline__ unsigned append_running(const PassArgs& p, bool more,
   return q;
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_first(const BatchArgs a, const PassArgs p) {
+// MOM: the batch runs the Polyak or Nesterov variant (false: the default one, L.variant never changes)
+template <int MODE, bool MOM>
+__global__ void __launch_bounds__(PASS_THREADS, pass_blocks_per_sm(true, MOM))
+    k_gjk_first(const BatchArgs a, const PassArgs p) {
+  using Store = SlotStore<!MOM>;  // the pose in shared memory where the pass runs 4 blocks per SM
   __shared__ double store_rows[4 * 6 * PASS_THREADS];
-  const SlotStore ss{store_rows + threadIdx.x};
+  __shared__ double pose_rows[Store::rows * PASS_THREADS];
+  const Store ss{store_rows + threadIdx.x, pose_rows + threadIdx.x};
   const unsigned lo = *a.range_lo, hi = *a.range_hi;
   const unsigned stride = gridDim.x * blockDim.x;
-  const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned k0 = lo + blockIdx.x * blockDim.x; k0 < hi; k0 += stride) {  // (warp-uniform trip count)
     const unsigned k = k0 + threadIdx.x;
     bool more = false, fin = false;
     unsigned i = 0;
-    double ssr0 = 0, ssr1 = 0;
     GjkStateT<SVSlot> g;
     GjkLoop L;
     if (k < hi) {
@@ -240,35 +311,35 @@ __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_first(
         GjkSetup S;
         PairOut o;
         pair_gjk_begin<CAP_PRIM>(in, a.P, S, L, g, o);
-        ssr0 = S.md.ssr0;
-        ssr1 = S.md.ssr1;
+        ss.set_pose(S);
         more = true;
-        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
+        for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM, Store, MOM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
         fin = !more;
       }
     }
     // the pairs that ended are finished after the others are saved: the loop state is dead by then
     if (p.out_list) {
       const unsigned q = append_running(p, more, k - lo);
-      if (more) save_running(p.rout, p.st.stride, q, g, L, momentum, ss);
+      if (more) save_running(p.rout, p.st.stride, q, g, L, MOM, ss);
     }
-    if (fin) finish_pair<MODE>(a, i, g, ss, ssr0, ssr1);
+    if (fin) finish_pair<MODE>(a, i, g, ss);
   }
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_more(const BatchArgs a, const PassArgs p) {
+template <int MODE, bool MOM>
+__global__ void __launch_bounds__(PASS_THREADS, pass_blocks_per_sm(false, MOM))
+    k_gjk_more(const BatchArgs a, const PassArgs p) {
+  using Store = SlotStore<false>;
   __shared__ double store_rows[4 * 6 * PASS_THREADS];
-  const SlotStore ss{store_rows + threadIdx.x};
+  __shared__ double pose_rows[Store::rows * PASS_THREADS];
+  const Store ss{store_rows + threadIdx.x, pose_rows + threadIdx.x};
   const unsigned lo = *a.range_lo;
   const unsigned n = *p.in_count;
   const unsigned stride = gridDim.x * blockDim.x;
-  const bool momentum = a.P.gjk.variant != HFB_GJK_DEFAULT;
   for (unsigned q0 = blockIdx.x * blockDim.x; q0 < n; q0 += stride) {
     const unsigned q = q0 + threadIdx.x;
     bool more = false;
     unsigned pos = 0, i = 0;
-    double ssr0 = 0, ssr1 = 0;
     GjkStateT<SVSlot> g;
     GjkLoop L;
     if (q < n) {
@@ -277,17 +348,16 @@ __global__ void __launch_bounds__(PASS_THREADS, PASS_BLOCKS_PER_SM) k_gjk_more(c
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       GjkSetup S;
       make_setup<CAP_PRIM>(in, S);
-      ssr0 = S.md.ssr0;
-      ssr1 = S.md.ssr1;
-      load_running(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L, ss);
+      ss.set_pose(S);
+      load_running<MOM>(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L, ss);
       more = true;
-      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
+      for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM, Store, MOM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
     }
     if (p.out_list) {
       const unsigned qo = append_running(p, more, pos);
-      if (more) save_running(p.rout, p.st.stride, qo, g, L, momentum, ss);
+      if (more) save_running(p.rout, p.st.stride, qo, g, L, MOM, ss);
     }
-    if (q < n && !more) finish_pair<MODE>(a, i, g, ss, ssr0, ssr1);
+    if (q < n && !more) finish_pair<MODE>(a, i, g, ss);
   }
 }
 
@@ -315,9 +385,9 @@ size_t gjk_pass_state_bytes(size_t n) {
 }
 
 // one block per PASS_THREADS pairs, at most 16 waves of resident blocks (the kernels stride over the rest)
-static unsigned pass_blocks(unsigned n, int num_sms) {
+static unsigned pass_blocks(unsigned n, int num_sms, bool first, bool mom) {
   unsigned blocks = (n + PASS_THREADS - 1) / PASS_THREADS;
-  const unsigned cap = (unsigned)num_sms * PASS_BLOCKS_PER_SM * 16u;
+  const unsigned cap = (unsigned)num_sms * pass_blocks_per_sm(first, mom) * 16u;
   if (blocks > cap) blocks = cap;
   return blocks ? blocks : 1u;
 }
@@ -329,7 +399,8 @@ int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint
   if (npass < 1) return (int)cudaErrorInvalidValue;
   cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)npass * sizeof(unsigned), s);
   if (e != cudaSuccess) return (int)e;
-  const unsigned blocks = pass_blocks(n, num_sms);
+  const bool mom = a.P.gjk.variant != HFB_GJK_DEFAULT;
+  const unsigned blocks = pass_blocks(n, num_sms, true, mom);
   PassArgs p;
   carve(state, n, p.st);
   p.in_list = nullptr;
@@ -338,8 +409,8 @@ int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint
   p.out_count = counts;
   p.rout = p.st.run[0];
   p.steps = npass > 1 ? steps[0] : 0x7fffffff;
-  if (mode == 0) k_gjk_first<0><<<blocks, PASS_THREADS, 0, s>>>(a, p);
-  else k_gjk_first<1><<<blocks, PASS_THREADS, 0, s>>>(a, p);
+  if (mode == 0) (mom ? k_gjk_first<0, true> : k_gjk_first<0, false>)<<<blocks, PASS_THREADS, 0, s>>>(a, p);
+  else (mom ? k_gjk_first<1, true> : k_gjk_first<1, false>)<<<blocks, PASS_THREADS, 0, s>>>(a, p);
   *launches += 1;
   return (int)cudaGetLastError();
 }
@@ -348,7 +419,8 @@ int gjk_passes_first(const BatchArgs& a, int mode, unsigned n, void* state, uint
 int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint32_t* list_a, uint32_t* list_b,
                     unsigned* counts, const int* steps, int npass, int num_sms, cudaStream_t s, int* launches) {
   if (npass < 2) return 0;
-  const unsigned blocks = pass_blocks(n, num_sms);
+  const bool mom = a.P.gjk.variant != HFB_GJK_DEFAULT;
+  const unsigned blocks = pass_blocks(n, num_sms, false, mom);
   PassArgs p;
   carve(state, n, p.st);
   for (int k = 1; k < npass; ++k) {
@@ -363,11 +435,11 @@ int gjk_passes_rest(const BatchArgs& a, int mode, unsigned n, void* state, uint3
     p.steps = last ? 0x7fffffff : steps[k];
     // the number of running pairs is only known on the device: the grid is sized for the typical survival rate of
     // a pass and strides over whatever there is, but never fills less than one wave of resident blocks
-    const unsigned wave = (unsigned)num_sms * PASS_BLOCKS_PER_SM;
+    const unsigned wave = (unsigned)num_sms * pass_blocks_per_sm(false, mom);
     unsigned b = blocks >> (k < 3 ? k : 3);
     if (b < wave) b = wave < blocks ? wave : blocks;
-    if (mode == 0) k_gjk_more<0><<<b, PASS_THREADS, 0, s>>>(a, p);
-    else k_gjk_more<1><<<b, PASS_THREADS, 0, s>>>(a, p);
+    if (mode == 0) (mom ? k_gjk_more<0, true> : k_gjk_more<0, false>)<<<b, PASS_THREADS, 0, s>>>(a, p);
+    else (mom ? k_gjk_more<1, true> : k_gjk_more<1, false>)<<<b, PASS_THREADS, 0, s>>>(a, p);
     ++*launches;
   }
   return (int)cudaGetLastError();

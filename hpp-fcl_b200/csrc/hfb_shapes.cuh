@@ -284,5 +284,19 @@ HFB_HD void mink_support(const ShapeD& s0, const ShapeD& s1, const MinkD& md, v3
     w1 = mmul(md.oR1, w1) + md.ot1;
   }
 }
+// The same, with what a pair's iterations never write -- the relative pose oR1 / ot1 and the shapes' parameters --
+// read from `mr` (the GJK passes keep them in a per-thread store in shared memory, SlotStore in hfb_gjkpass.cu).  The
+// pose is read once before the second support call and once after it, so that it is not live across the call.
+template <int G, int CAPS, class Mink>
+HFB_HD void mink_support(const ShapeD& s0, const ShapeD& s1, const MinkD& md, v3 dir, v3& w0, v3& w1,
+                         int& hint0, int& hint1, const Mink& mr) {
+  w0 = shape_support<G, CAPS>(mr.shape0(s0), dir, hint0);
+  if (md.identity) {
+    w1 = shape_support<G, CAPS>(mr.shape1(s1), -dir, hint1);
+  } else {
+    w1 = shape_support<G, CAPS>(mr.shape1(s1), -mtmul(mr.oR1(), dir), hint1);
+    w1 = mmul(mr.oR1(), w1) + mr.ot1();
+  }
+}
 
 }  // namespace hfb
