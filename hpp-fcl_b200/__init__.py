@@ -16,5 +16,5 @@ from .api import (  # noqa: F401
     BVHModelOBB, BVHModelOBBRSS, Box, Capsule, CollisionRequest, CollisionResult, Cone, Contact, Convex, Cylinder,
     DistanceRequest, DistanceResult, Ellipsoid, Halfspace, Plane, Sphere, Transform3f, TriangleP,
     collide, distance, ComputeCollision, ComputeDistance, BatchQuery,
-    AABB, CollisionObject, CollisionCallBackCollect, DynamicAABBTreeCollisionManager,
+    AABB, CollisionObject, CollisionCallBackCollect, DynamicAABBTreeCollisionManager, ResidentEnvironment,
 )

@@ -154,6 +154,10 @@ class SceneContacts(C.Structure):
                 ("n_colliding", C.c_void_p), ("n_candidates", C.c_void_p)]
 
 
+class EnvOut(C.Structure):  # hfb_env_out: hfb_scene_contacts + one flag byte per A object
+    _fields_ = SceneContacts._fields_ + [("flags", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -568,8 +568,24 @@ class DynamicAABBTreeCollisionManager:
     def setup(self):
         self._refresh()
 
-    def update(self):
-        self._refresh()
+    def update(self, objs=None):
+        """update(): every object's box again; update(obj) / update(objs): the boxes of those objects from their current
+        poses (broadphase_collision_manager.h:76-79)"""
+        if objs is None or self._stale:
+            self._refresh()
+            return
+        if isinstance(objs, CollisionObject):
+            objs = [objs]
+        where = {id(o): i for i, o in enumerate(self.objs)}
+        objs = [o for o in objs if id(o) in where]  # an object the manager does not hold is skipped, as the reference does
+        idx = np.array([where[id(o)] for o in objs], dtype=np.int64)
+        if idx.size == 0:
+            return
+        self._tfs[idx] = _tf_array([o.tf for o in objs])
+        bb = self.scene.engine.scene_aabbs(self._handles[idx], self._tfs[idx])
+        self._boxes[idx] = bb
+        for o, b in zip(objs, bb):
+            o.aabb = AABB(b[:3].copy(), b[3:].copy())
 
     def _table(self, other):
         """(handles, poses, boxes, objects) of `other`: another manager (refreshed if stale) or one CollisionObject,
@@ -639,6 +655,70 @@ class DynamicAABBTreeCollisionManager:
         rec = self.scene.engine.batch_collide_objects(np.concatenate([self._handles, hb]), np.concatenate([self._tfs, tb]),
                                                       first, second + np.uint32(n), request._pod)
         return first, second, rec
+
+
+class ResidentEnvironment:
+    """A manager's objects kept on the device as set B of the two-set collide (hfb_env): its table, its boxes as of
+    construction / update(objs) and the grid over them stay there between queries, as the reference's tree does between
+    setup() and update().  collide() and collide_flags() upload only the robot manager's poses.  close() (or leaving a
+    `with` block) frees it."""
+
+    def __init__(self, manager):
+        if manager._stale:
+            manager._refresh()
+        self.engine = manager.scene.engine
+        self._index = {id(o): i for i, o in enumerate(manager.objs)}
+        self._env = self.engine.env_create(manager._handles, manager._tfs)
+
+    def update(self, objs):
+        """the current poses of these environment objects (one CollisionObject or several) pushed to the device"""
+        if isinstance(objs, CollisionObject):
+            objs = [objs]
+        if any(id(o) not in self._index for o in objs):  # (the C++ mirror throws std::invalid_argument)
+            raise ValueError("not an object of this environment")
+        idx = np.array([self._index[id(o)] for o in objs], dtype=np.uint32)
+        tfs = _tf_array([o.tf for o in objs]) if len(objs) else np.zeros(0, dtype=P.transform_dtype)
+        self.engine.env_update(self._env, idx, tfs)
+
+    @staticmethod
+    def _robot(robot_manager, request):
+        request = request or CollisionRequest()
+        if request.num_max_contacts == 0 and request.security_margin != -np.inf:
+            raise ValueError("Invalid number of max contacts (current value is 0).")
+        if robot_manager._stale:
+            robot_manager._refresh()
+        return robot_manager._handles, robot_manager._tfs, request._pod
+
+    def collide(self, robot_manager, request=None, capacity=None):
+        """-> (first = index in the robot manager, second = index in the environment, contact records) of the colliding
+        pairs, in no particular order"""
+        h, t, req = self._robot(robot_manager, request)
+        first, second, rec, _, hits = self.engine.env_collide(self._env, h, t, req, capacity=capacity)
+        if capacity is None and hits > len(first):  # (all of them unless a capacity is given)
+            first, second, rec, _, _ = self.engine.env_collide(self._env, h, t, req, capacity=hits)
+        return first, second, rec
+
+    def collide_flags(self, robot_manager, request=None):
+        """-> one byte per robot object: 1 iff it collides with the environment (no pair records come back)"""
+        h, t, req = self._robot(robot_manager, request)
+        return self.engine.env_collide(self._env, h, t, req, capacity=0, flags=True)[5]
+
+    def close(self):
+        if getattr(self, "_env", None) is not None and getattr(self.engine, "h", None):
+            self.engine.env_destroy(self._env)
+        self._env = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def _unsupported(o1, o2, what, request=None):

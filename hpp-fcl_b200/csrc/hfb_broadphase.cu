@@ -13,12 +13,9 @@ namespace {
 
 constexpr unsigned kMaxCells = 2097152u;
 
-__global__ void __launch_bounds__(256) k_scene_aabbs(const double* local, uint32_t nshapes, unsigned n,
-                                                     const uint32_t* handles, const hfb_transform* tfs, double* out) {
-  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t h = handles[i];
-  double* o = out + 6 * (size_t)i;
+// world-space box of one object (k_scene_aabbs, k_env_update)
+__device__ __forceinline__ void scene_aabb(const double* local, uint32_t nshapes, uint32_t h, const hfb_transform& tf,
+                                           double* o) {
   if (h >= nshapes) {  // no such geometry: an empty box that overlaps nothing
     for (int k = 0; k < 3; ++k) {
       o[k] = DBL_MAX;
@@ -34,7 +31,24 @@ __global__ void __launch_bounds__(256) k_scene_aabbs(const double* local, uint32
     }
     return;
   }
-  object_aabb(l, l + 3, tfs[i], o);
+  object_aabb(l, l + 3, tf, o);
+}
+__global__ void __launch_bounds__(256) k_scene_aabbs(const double* local, uint32_t nshapes, unsigned n,
+                                                     const uint32_t* handles, const hfb_transform* tfs, double* out) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  scene_aabb(local, nshapes, handles[i], tfs[i], out + 6 * (size_t)i);
+}
+// hfb_env_update: m new poses scattered into the resident table (index idx[k] of B), and those m boxes recomputed
+__global__ void __launch_bounds__(256) k_env_update(const double* local, uint32_t nshapes, unsigned m, const uint32_t* idx,
+                                                    const hfb_transform* tfs_new, const uint32_t* handles,
+                                                    hfb_transform* tfs, double* bb) {
+  const unsigned k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= m) return;
+  const unsigned i = idx[k];
+  const hfb_transform tf = tfs_new[k];
+  tfs[i] = tf;
+  scene_aabb(local, nshapes, handles[i], tf, bb + 6 * (size_t)i);
 }
 
 struct Bounds {  // centres' box and the largest extent
@@ -364,6 +378,33 @@ __global__ void __launch_bounds__(128) k_cross_brute(const double* ba, const dou
   }
 }
 
+// the resident environment's query: the A objects k_cross_sweep handles (in range, with a box, not on the brute list)
+// against B's oversize and unbounded objects (the end of `order`), one thread per pair -- k_cross_sweep's own loop over
+// that list is one serial chain per A object, which a few configurations against a list of about a thousand tables
+// cannot hide
+__global__ void __launch_bounds__(128) k_cross_oversize(const double* ba, unsigned a_lo, unsigned a_hi, const double* bb,
+                                                        unsigned nb, const CrossGrid* cgp, const unsigned* order,
+                                                        const unsigned* counters, uint32_t* first, uint32_t* second,
+                                                        unsigned second_base, unsigned capacity, unsigned* n_pairs) {
+  const unsigned na = a_hi - a_lo;
+  const size_t total = (size_t)na * counters[0];
+  const size_t tend = (total + 31u) & ~(size_t)31;  // (warp-uniform trip count for the ballots)
+  const CrossGrid cg = *cgp;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < tend; t += (size_t)gridDim.x * blockDim.x) {
+    bool hit = false;
+    unsigned i = 0, u = 0;
+    if (t < total) {
+      i = a_lo + (unsigned)(t % na);
+      u = order[nb - 1u - (unsigned)(t / na)];
+      const double* a = ba + 6 * (size_t)i;
+      int c0[3], c1[3];
+      hit = !aabb_empty(a) && !aabb_unbounded(a) && cross_query_cells(cg.g, cg.cell, a, c0, c1) <= kCrossScanRows &&
+            aabb_overlap(a, bb + 6 * (size_t)u);
+    }
+    append_pair(hit, i, u + second_base, first, second, capacity, n_pairs);
+  }
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -454,41 +495,135 @@ size_t bp_cross_scratch_bytes(size_t n_a, size_t n_b) {
   return bp_scratch_bytes(n_b) + up256((size_t)kExtBins * 4) + up256(n_a * 4);
 }
 
-int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
-                          uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity, unsigned* d_n_pairs,
-                          void* scratch, int num_sms, cudaStream_t s, int* launches) {
-  if (num_sms < 1) num_sms = 1;
+namespace {
+// the grid over B in two steps: its bounds, cell and dims (clearing *d_n_pairs and both counters), then B's objects
+// binned into `order` / `start` (the oversize and unbounded ones listed from the end of `order`)
+int cross_grid_fit(size_t n_b, const double* d_aabbs_b, const BpCrossGrid& g, unsigned* d_n_pairs, void* scratch,
+                   cudaStream_t s, int* launches) {
   Scratch w = carve(scratch, n_b);
-  unsigned char* extra = static_cast<unsigned char*>(scratch) + bp_scratch_bytes(n_b);
-  unsigned* hist = reinterpret_cast<unsigned*>(extra);
-  unsigned* brute = reinterpret_cast<unsigned*>(extra + up256((size_t)kExtBins * 4));
-  CrossGrid* cg = reinterpret_cast<CrossGrid*>(w.grid);  // (the grid slot has 256 bytes)
-  unsigned* counters = w.n_unbounded;                    // [0]: B oversize + unbounded, [1]: A brute
+  unsigned* hist = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(scratch) + bp_scratch_bytes(n_b));
   const unsigned nb = (unsigned)n_b;
-  const unsigned cap = (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity);
   unsigned pb = (nb + 255) / 256;
   if (pb > kParts) pb = kParts;
   if (pb == 0) pb = 1;
   cudaError_t e;
   if ((e = cudaMemsetAsync(hist, 0, (size_t)kExtBins * 4, s)) != cudaSuccess) return (int)e;
   k_cross_bounds_partial<<<pb, 256, 0, s>>>(d_aabbs_b, nb, w.part, hist);
-  k_cross_grid<<<1, 256, 0, s>>>(w.part, pb, hist, cg, d_n_pairs, counters);
+  k_cross_grid<<<1, 256, 0, s>>>(w.part, pb, hist, static_cast<CrossGrid*>(g.grid), d_n_pairs, g.counters);
   *launches += 2;
-  if (a_hi > n_a) a_hi = n_a;
-  if (n_b == 0 || a_lo >= a_hi) return (int)cudaGetLastError();
+  return (int)cudaGetLastError();
+}
+int cross_grid_bin(size_t n_b, const double* d_aabbs_b, const BpCrossGrid& g, void* scratch, cudaStream_t s, int* launches) {
+  Scratch w = carve(scratch, n_b);
+  CrossGrid* cg = static_cast<CrossGrid*>(g.grid);
+  const unsigned nb = (unsigned)n_b;
+  cudaError_t e;
   if ((e = cudaMemsetAsync(w.count, 0, (size_t)(kMaxCells + 1) * 4, s)) != cudaSuccess) return (int)e;
   if ((e = cudaMemsetAsync(w.cursor, 0, (size_t)kMaxCells * 4, s)) != cudaSuccess) return (int)e;
-  k_cell_hist<<<(nb + 255) / 256, 256, 0, s>>>(d_aabbs_b, nb, &cg->g, w.cell, w.count, w.order, counters, &cg->cell);
+  k_cell_hist<<<(nb + 255) / 256, 256, 0, s>>>(d_aabbs_b, nb, &cg->g, w.cell, w.count, g.order, g.counters, &cg->cell);
   size_t tb = w.cub_bytes;
-  if ((e = cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, w.count, w.start, (int)(kMaxCells + 1), s)) != cudaSuccess) return (int)e;
-  k_cell_scatter<<<(nb + 255) / 256, 256, 0, s>>>(w.cell, nb, w.start, w.cursor, w.order);
-  k_cross_sweep<<<(unsigned)((a_hi - a_lo + 127) / 128), 128, 0, s>>>(d_aabbs_a, (unsigned)a_lo, (unsigned)a_hi, d_aabbs_b, nb, cg,
-                                                                      w.start, w.order, counters, brute, d_first, d_second,
-                                                                      second_base, cap, d_n_pairs);
+  if ((e = cub::DeviceScan::ExclusiveSum(w.cub_tmp, tb, w.count, g.start, (int)(kMaxCells + 1), s)) != cudaSuccess) return (int)e;
+  k_cell_scatter<<<(nb + 255) / 256, 256, 0, s>>>(w.cell, nb, g.start, w.cursor, g.order);
+  *launches += 3;
+  return (int)cudaGetLastError();
+}
+}  // namespace
+
+size_t bp_cross_grid_bytes(size_t n_b) { return 512 + up256(n_b * 4) + up256((size_t)(kMaxCells + 1) * 4); }
+
+BpCrossGrid bp_cross_grid_carve(void* p, size_t n_b) {
+  unsigned char* c = static_cast<unsigned char*>(p);
+  BpCrossGrid g;
+  g.grid = c;
+  g.counters = reinterpret_cast<unsigned*>(c + 256);
+  g.order = reinterpret_cast<unsigned*>(c + 512);
+  g.start = reinterpret_cast<unsigned*>(c + 512 + up256(n_b * 4));
+  return g;
+}
+
+int bp_cross_build_launch(size_t n_b, const double* d_aabbs_b, const BpCrossGrid& g, void* scratch, cudaStream_t s,
+                          int* launches) {
+  // (k_cross_grid clears a pair counter: the one of the next query is cleared by bp_cross_query_reset)
+  if (int e = cross_grid_fit(n_b, d_aabbs_b, g, g.counters + 2, scratch, s, launches)) return e;
+  return n_b ? cross_grid_bin(n_b, d_aabbs_b, g, scratch, s, launches) : 0;
+}
+
+namespace {
+// the grid rows of every A object in [a_lo, a_hi) (k_cross_sweep) and the A objects that need all of B (k_cross_brute);
+// counters[0]: the length of B's oversize list k_cross_sweep walks, counters[1]: the length of A's brute list
+int cross_sweep(size_t a_lo, size_t a_hi, const double* d_aabbs_a, size_t n_b, const double* d_aabbs_b, const BpCrossGrid& g,
+                unsigned* counters, uint32_t* d_first, uint32_t* d_second, uint32_t second_base, unsigned cap,
+                unsigned* d_n_pairs, void* scratch, int num_sms, cudaStream_t s, int* launches) {
+  unsigned* brute = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(scratch) + bp_scratch_bytes(n_b) +
+                                                up256((size_t)kExtBins * 4));
+  const unsigned nb = (unsigned)n_b;
+  k_cross_sweep<<<(unsigned)((a_hi - a_lo + 127) / 128), 128, 0, s>>>(d_aabbs_a, (unsigned)a_lo, (unsigned)a_hi, d_aabbs_b, nb,
+                                                                      static_cast<const CrossGrid*>(g.grid), g.start, g.order,
+                                                                      counters, brute, d_first, d_second, second_base, cap,
+                                                                      d_n_pairs);
   unsigned ub = (nb + 127) / 128;
   if (ub > (unsigned)num_sms * 8u) ub = (unsigned)num_sms * 8u;
   k_cross_brute<<<ub, 128, 0, s>>>(d_aabbs_a, d_aabbs_b, nb, counters, brute, d_first, d_second, second_base, cap, d_n_pairs);
-  *launches += 5;
+  *launches += 2;
+  return (int)cudaGetLastError();
+}
+}  // namespace
+
+// A query against a built grid reads its counters from g.counters + 2: [2] stays 0 (k_cross_grid cleared it at the
+// build), so k_cross_sweep leaves B's oversize list to k_cross_oversize, which reads its length from [0]; [3] is A's
+// brute list
+int bp_cross_query_reset(const BpCrossGrid& g, unsigned* d_n_pairs, cudaStream_t s) {
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(d_n_pairs, 0, sizeof(unsigned), s)) != cudaSuccess) return (int)e;
+  return (int)cudaMemsetAsync(g.counters + 3, 0, sizeof(unsigned), s);  // A's brute list; B's oversize count stays
+}
+
+int bp_cross_query_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
+                          const BpCrossGrid& g, uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity,
+                          unsigned* d_n_pairs, void* scratch, int num_sms, cudaStream_t s, int* launches) {
+  if (num_sms < 1) num_sms = 1;
+  if (a_hi > n_a) a_hi = n_a;
+  if (n_b == 0 || a_lo >= a_hi) return 0;
+  const unsigned cap = (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity);
+  if (int e = cross_sweep(a_lo, a_hi, d_aabbs_a, n_b, d_aabbs_b, g, g.counters + 2, d_first, d_second, second_base, cap,
+                          d_n_pairs, scratch, num_sms, s, launches))
+    return e;
+  // (grid-stride: the length of the list is only known on the device)
+  size_t ob = ((a_hi - a_lo) * n_b + 127) / 128;
+  if (ob > (size_t)num_sms * 16u) ob = (size_t)num_sms * 16u;
+  k_cross_oversize<<<(unsigned)ob, 128, 0, s>>>(d_aabbs_a, (unsigned)a_lo, (unsigned)a_hi, d_aabbs_b, (unsigned)n_b,
+                                                static_cast<const CrossGrid*>(g.grid), g.order, g.counters, d_first, d_second,
+                                                second_base, cap, d_n_pairs);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
+                          uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity, unsigned* d_n_pairs,
+                          void* scratch, int num_sms, cudaStream_t s, int* launches) {
+  if (num_sms < 1) num_sms = 1;
+  // the grid in the self form's slots of the scratch: grid (256 bytes), counters ([0]: B oversize + unbounded, [1]: A
+  // brute), order, start
+  Scratch w = carve(scratch, n_b);
+  BpCrossGrid g;
+  g.grid = w.grid;
+  g.counters = w.n_unbounded;
+  g.order = w.order;
+  g.start = w.start;
+  if (int e = cross_grid_fit(n_b, d_aabbs_b, g, d_n_pairs, scratch, s, launches)) return e;
+  if (a_hi > n_a) a_hi = n_a;
+  if (n_b == 0 || a_lo >= a_hi) return 0;
+  if (int e = cross_grid_bin(n_b, d_aabbs_b, g, scratch, s, launches)) return e;
+  return cross_sweep(a_lo, a_hi, d_aabbs_a, n_b, d_aabbs_b, g, g.counters, d_first, d_second, second_base,
+                     (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity), d_n_pairs, scratch, num_sms, s, launches);
+}
+
+int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
+                         const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,
+                         cudaStream_t s) {
+  if (m == 0) return 0;
+  k_env_update<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(d_local_aabbs, nshapes, (unsigned)m, d_idx, d_tfs_new, d_handles,
+                                                           d_tfs, d_aabbs);
   return (int)cudaGetLastError();
 }
 

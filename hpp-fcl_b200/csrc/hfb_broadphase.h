@@ -28,4 +28,29 @@ int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size
                           uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity, unsigned* d_n_pairs,
                           void* scratch, int num_sms, cudaStream_t s, int* launches);
 
+// bp_cross_pairs_launch in its two halves, for a grid over B that outlives the call (hfb_env): the grid's persistent
+// part -- cell size and dims, B's oversize count, `order`, `start` -- lives in bp_cross_grid_bytes(n_b) bytes of the
+// caller's; the build-only buffers and A's brute list come from `scratch` (bp_cross_scratch_bytes(n_a, n_b) bytes).
+struct BpCrossGrid {
+  void* grid;          // cell size and dims (256 bytes)
+  unsigned* counters;  // [0]: B's oversize + unbounded objects; [2], [3]: a query's (bp_cross_query_reset)
+  unsigned* order;     // n_b
+  unsigned* start;     // cells + 1
+};
+size_t bp_cross_grid_bytes(size_t n_b);
+BpCrossGrid bp_cross_grid_carve(void* p, size_t n_b);
+// the grid over B's boxes; run again after B's boxes change
+int bp_cross_build_launch(size_t n_b, const double* d_aabbs_b, const BpCrossGrid& g, void* scratch, cudaStream_t s,
+                          int* launches);
+// clears *d_n_pairs and A's brute list (not B's oversize count) in front of a query against a built grid
+int bp_cross_query_reset(const BpCrossGrid& g, unsigned* d_n_pairs, cudaStream_t s);
+// the query: k_cross_sweep and k_cross_brute as in bp_cross_pairs_launch, B's oversize list by k_cross_oversize
+int bp_cross_query_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
+                          const BpCrossGrid& g, uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity,
+                          unsigned* d_n_pairs, void* scratch, int num_sms, cudaStream_t s, int* launches);
+// hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
+int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
+                         const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,
+                         cudaStream_t s);
+
 }  // namespace hfb

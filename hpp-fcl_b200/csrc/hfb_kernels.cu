@@ -22,7 +22,9 @@
 
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -697,6 +699,22 @@ __global__ void __launch_bounds__(256) k_compact_scene(const hfb_contact* r, con
     recs[pos] = r[i];
   }
 }
+// hfb_env_collide's flags: the A object of a colliding candidate gets flag 1 (every writer stores the same byte);
+// count (null: not counted) gets the number of colliding candidates when no compaction counts them
+__global__ void __launch_bounds__(256) k_flag_colliding(const hfb_contact* r, const uint32_t* pf, unsigned n, uint8_t* flags,
+                                                        unsigned* count) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool hit = i < n && r[i].num_contacts > 0;
+  if (hit) flags[pf[i]] = 1;
+  if (!count) return;
+  const unsigned m = __ballot_sync(0xffffffffu, hit);
+  if (m && (threadIdx.x & 31u) == 0) atomicAdd(count, (unsigned)__popc(m));
+}
+// hfb_env_collide_device: the compacted second indices from the table [A; B] back into B (the count is on the device)
+__global__ void __launch_bounds__(256) k_unbase(uint32_t* second, const unsigned* count, unsigned cap, uint32_t base) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < *count && i < cap) second[i] -= base;
+}
 
 // ----------------------------------------------------- convex support kernel --
 // One warp per query: streams the SoA vertex block (coalesced 256-B rows) and
@@ -872,8 +890,26 @@ struct hfb_ctx {
   unsigned comm_calls = 0;
   DevBuf bp_scratch;                // device broadphase
   DevBuf sc_bb, sc_pf, sc_ps, sc_cnt, sc_out, sc_f, sc_s, sc_rec;  // hfb_scene_collide
+  DevBuf sc_flags;                                                 // hfb_env_collide
+  // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
+  std::vector<hfb_env*> envs;
+  uint64_t commits = 0, clears = 0;
   std::string err;
   std::mutex mu;
+};
+
+// set B on the device (hfb_env_create): the object table with `head` free slots in front of B for A, so that a query's
+// table [A; B] is contiguous without copying B; B's boxes and the persistent part of the cross grid over them
+struct hfb_env {
+  size_t n_b = 0, head = 0;
+  DevBuf h, tf;  // (head + n_b) handles and poses, B from slot `head` on
+  DevBuf bb;     // B's boxes
+  DevBuf grid;   // hfb::bp_cross_grid_bytes(n_b)
+  std::vector<uint32_t> handles;  // B's handles, checked again after a commit
+  uint64_t commits = 0, clears = 0;  // the context's counters when B was last checked
+  ~hfb_env() {
+    for (DevBuf* b : {&h, &tf, &bb, &grid}) b->release();
+  }
 };
 
 namespace {
@@ -1910,7 +1946,9 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   if (c->pin_fix) cudaFreeHost(c->pin_fix);
   for (cudaEvent_t e : c->pipe_events) cudaEventDestroy(e);
   c->bp_scratch.release();
-  for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec}) b->release();
+  for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec, &c->sc_flags})
+    b->release();
+  for (hfb_env* e : c->envs) delete e;
   c->obj_tf.release();
   c->cmp_flags.release();
   c->cmp_count.release();
@@ -2044,6 +2082,7 @@ int hfb_geom_commit(hfb_ctx* ctx) {
     ctx->dview.local_aabbs = reinterpret_cast<const double*>(pl);
   }
   ctx->committed = true;
+  ++ctx->commits;
   return HFB_OK;
 }
 
@@ -2063,6 +2102,7 @@ int hfb_geom_clear(hfb_ctx* ctx) {
   ctx->arena = HostArena();
   ctx->dview = ArenaView{};
   ctx->committed = false;
+  ++ctx->clears;
   return HFB_OK;
 }
 
@@ -2417,19 +2457,25 @@ int hfb_broadphase_pairs_device(hfb_ctx* ctx, size_t n, const double* d_aabbs, s
 
 }  // extern "C"
 
-// The part hfb_scene_collide and hfb_scene_collide_sets share, after the upload of the object table (d_h, d_tf: n
-// objects): the boxes, the candidates (find_pairs(d_bb, pf, ps, capacity, d_count, &launches) launches a pair finder,
-// all pairs counted in *d_count, at most `capacity` stored), collide() of every candidate over the table, compaction
-// and download; `second_base` is subtracted from the downloaded second indices.
+// the *_device calls may still be reading the shared scratch (the candidates, their records and counters of
+// hfb_env_collide_device) or an env's table on another stream: a call on stream s that writes them waits for them first
+static int after_device_calls(hfb_ctx* ctx, cudaStream_t s) {
+  if (ctx->dev_used && ctx->dev_last_stream != s) CK(cudaStreamWaitEvent(s, ctx->dev_done, 0));
+  return HFB_OK;
+}
+// The part hfb_scene_collide, hfb_scene_collide_sets and hfb_env_collide share, after the upload of the object table
+// (d_h, d_tf: n objects): the boxes of its first n_boxes objects, the candidates (find_pairs(d_bb, pf, ps, capacity,
+// d_count, &launches) launches a pair finder, all pairs counted in *d_count, at most `capacity` stored) and collide() of
+// every candidate over the table, into ctx->sc_out (none when there are no candidates or under minus_inf).
 template <class FindPairs>
-static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
-                               FindPairs find_pairs, uint32_t second_base, const hfb_collision_request* req, bool minus_inf,
-                               const hfb_scene_contacts* out) {
-  CK(ctx->sc_bb.reserve(n * 48));
+static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
+                            size_t n_boxes, FindPairs find_pairs, const hfb_collision_request* req, bool minus_inf,
+                            unsigned* cand_out) {
+  CK(ctx->sc_bb.reserve(n_boxes * 48));
   CK(ctx->sc_cnt.reserve(16));
   double* d_bb = static_cast<double*>(ctx->sc_bb.p);
   unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
-  if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n, d_h, d_tf, d_bb, s) != 0)
+  if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n_boxes, d_h, d_tf, d_bb, s) != 0)
     return fail(ctx, HFB_ERR_CUDA, "k_scene_aabbs launch failed");
   ctx->stats.kernel_launches++;
   // the number of candidate pairs is not known in advance: a first sweep counts, a second one (if the buffers were too
@@ -2449,12 +2495,9 @@ static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uin
     CK(ctx->sc_ps.reserve(cap * 4));
     cap = ctx->sc_pf.cap / 4 < ctx->sc_ps.cap / 4 ? ctx->sc_pf.cap / 4 : ctx->sc_ps.cap / 4;
   }
-  if (out->n_candidates) *out->n_candidates = cand;
+  *cand_out = cand;
   if (cand == 0 || minus_inf) return HFB_OK;  // collision.cpp:73-76: no contacts under security_margin == -inf
   CK(ctx->sc_out.reserve((size_t)cand * sizeof(hfb_contact)));
-  CK(ctx->sc_f.reserve((size_t)out->capacity * 4 + 4));
-  CK(ctx->sc_s.reserve((size_t)out->capacity * 4 + 4));
-  CK(ctx->sc_rec.reserve((size_t)out->capacity * sizeof(hfb_contact) + 8));
   hfb_object_pairs sc;
   sc.n_objects = n;
   sc.object_handles = d_h;
@@ -2463,29 +2506,85 @@ static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uin
   sc.first = static_cast<const uint32_t*>(ctx->sc_pf.p);
   sc.second = static_cast<const uint32_t*>(ctx->sc_ps.p);
   CollideP C{req->security_margin, req->q.collision_distance_threshold};
-  if (int rc = objects_device<1>(ctx, &sc, req, solver_from_collision_request(*req), C, bvh_req_of_collision(req), ctx->sc_out.p,
-                                 nullptr, s))
-    return rc;
+  return objects_device<1>(ctx, &sc, req, solver_from_collision_request(*req), C, bvh_req_of_collision(req), ctx->sc_out.p,
+                           nullptr, s);
+}
+
+// The colliding ones of scene_candidates' `cand` candidates: compacted (pairs and records, at most out->capacity; not
+// when out->flags is set and capacity is 0) and flagged per A object (out->flags, n_flags of them, when set).  dev: the
+// outputs are device memory, written on s; else host memory, downloaded.  `second_base` is subtracted from the second
+// indices.
+static int scene_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, uint32_t second_base, const hfb_env_out* out,
+                        size_t n_flags, bool dev) {
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+  const hfb_contact* recs = static_cast<const hfb_contact*>(ctx->sc_out.p);
+  const uint32_t* pf = static_cast<const uint32_t*>(ctx->sc_pf.p);
+  const bool compact = !out->flags || out->capacity;
   CK(cudaMemsetAsync(d_cnt + 1, 0, sizeof(unsigned), s));
-  k_compact_scene<<<(cand + 255) / 256, 256, 0, s>>>(static_cast<const hfb_contact*>(ctx->sc_out.p), sc.first, sc.second, cand,
-                                                      d_cnt + 1, static_cast<uint32_t*>(ctx->sc_f.p),
-                                                      static_cast<uint32_t*>(ctx->sc_s.p), static_cast<hfb_contact*>(ctx->sc_rec.p),
-                                                      out->capacity);
-  ctx->stats.kernel_launches++;
+  uint8_t* flags = out->flags;
+  if (flags) {
+    if (!dev) {
+      CK(ctx->sc_flags.reserve(n_flags));
+      flags = static_cast<uint8_t*>(ctx->sc_flags.p);
+    }
+    CK(cudaMemsetAsync(flags, 0, n_flags, s));
+    k_flag_colliding<<<(cand + 255) / 256, 256, 0, s>>>(recs, pf, cand, flags, compact ? nullptr : d_cnt + 1);
+    ctx->stats.kernel_launches++;
+  }
+  uint32_t *first = out->first, *second = out->second;
+  hfb_contact* contacts = out->contacts;
+  if (compact) {
+    if (!dev) {
+      CK(ctx->sc_f.reserve((size_t)out->capacity * 4 + 4));
+      CK(ctx->sc_s.reserve((size_t)out->capacity * 4 + 4));
+      CK(ctx->sc_rec.reserve((size_t)out->capacity * sizeof(hfb_contact) + 8));
+      first = static_cast<uint32_t*>(ctx->sc_f.p);
+      second = static_cast<uint32_t*>(ctx->sc_s.p);
+      contacts = static_cast<hfb_contact*>(ctx->sc_rec.p);
+    }
+    k_compact_scene<<<(cand + 255) / 256, 256, 0, s>>>(recs, pf, static_cast<const uint32_t*>(ctx->sc_ps.p), cand, d_cnt + 1,
+                                                        first, second, contacts, out->capacity);
+    ctx->stats.kernel_launches++;
+  }
+  if (dev) {
+    const unsigned most = cand < out->capacity ? cand : out->capacity;
+    if (compact && second_base && most) {
+      k_unbase<<<(most + 255) / 256, 256, 0, s>>>(out->second, d_cnt + 1, out->capacity, second_base);
+      ctx->stats.kernel_launches++;
+    }
+    if (out->n_colliding) CK(cudaMemcpyAsync(out->n_colliding, d_cnt + 1, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
+    CK(cudaGetLastError());
+    return HFB_OK;
+  }
   unsigned hits = 0;
   CK(cudaMemcpyAsync(&hits, d_cnt + 1, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (out->n_colliding) *out->n_colliding = hits;
-  const unsigned kept = hits < out->capacity ? hits : out->capacity;
+  const unsigned kept = !compact ? 0u : hits < out->capacity ? hits : out->capacity;
   if (kept) {
-    CK(cudaMemcpyAsync(out->first, ctx->sc_f.p, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(out->second, ctx->sc_s.p, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(out->contacts, ctx->sc_rec.p, (size_t)kept * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    if (second_base)
-      for (unsigned k = 0; k < kept; ++k) out->second[k] -= second_base;
+    CK(cudaMemcpyAsync(out->first, first, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(out->second, second, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(out->contacts, contacts, (size_t)kept * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
   }
+  if (flags) CK(cudaMemcpyAsync(out->flags, flags, n_flags, cudaMemcpyDeviceToHost, s));
+  if (kept || flags) CK(cudaStreamSynchronize(s));
+  if (second_base)
+    for (unsigned k = 0; k < kept; ++k) out->second[k] -= second_base;
   return HFB_OK;
+}
+
+// hfb_scene_collide and hfb_scene_collide_sets: boxes of the whole table, candidates, narrow phase, compaction and
+// download
+template <class FindPairs>
+static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
+                               FindPairs find_pairs, uint32_t second_base, const hfb_collision_request* req, bool minus_inf,
+                               const hfb_scene_contacts* out) {
+  unsigned cand = 0;
+  if (int rc = scene_candidates(ctx, s, n, d_h, d_tf, n, find_pairs, req, minus_inf, &cand)) return rc;
+  if (out->n_candidates) *out->n_candidates = cand;
+  if (cand == 0 || minus_inf) return HFB_OK;
+  const hfb_env_out o{out->first, out->second, out->contacts, out->capacity, out->n_colliding, nullptr, nullptr};
+  return scene_output(ctx, s, cand, second_base, &o, 0, false);
 }
 
 extern "C" {
@@ -2509,6 +2608,7 @@ int hfb_scene_collide(hfb_ctx* ctx, size_t n, const uint32_t* handles, const hfb
   if (n < 2) return HFB_OK;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
   CK(ctx->obj_h.reserve(n * 4 + 4));
   CK(ctx->obj_tf.reserve(n * sizeof(hfb_transform) + 8));
   CK(ctx->bp_scratch.reserve(bp_scratch_bytes(n)));
@@ -2574,6 +2674,7 @@ int hfb_scene_collide_sets(hfb_ctx* ctx, size_t n_a, const uint32_t* handles_a, 
   const size_t n = n_a + n_b;
   CK(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
   CK(ctx->obj_h.reserve(n * 4 + 4));
   CK(ctx->obj_tf.reserve(n * sizeof(hfb_transform) + 8));
   CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
@@ -2589,6 +2690,222 @@ int hfb_scene_collide_sets(hfb_ctx* ctx, size_t n_a, const uint32_t* handles_a, 
                                  ctx->bp_scratch.p, ctx->num_sms, s, nl);
   };
   return scene_collide_table(ctx, s, n, d_h, d_tf, find, (uint32_t)n_a, req, minus_inf, out);
+}
+
+}  // extern "C"
+
+// ---- resident environment (hfb_env): set B's table, boxes and cross grid kept on the device ----------------------
+// an env of this context whose B is still valid: the geometry was not cleared since its creation, and after a commit
+// B's handles are checked again (in range, not released)
+static int env_ready(hfb_ctx* ctx, hfb_env* e) {
+  if (std::find(ctx->envs.begin(), ctx->envs.end(), e) == ctx->envs.end())
+    return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "not an environment of this context");
+  if (e->clears != ctx->clears)
+    return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "the geometry was cleared since the environment was created (hfb_geom_clear)");
+  if (int rc = check_ready(ctx)) return rc;
+  if (e->commits != ctx->commits) {
+    if (int rc = check_handles(ctx, e->handles.data(), e->n_b)) return rc;
+    for (uint32_t h : e->handles)
+      if (ctx->arena.shapes[h].type == 0) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "a shape of the environment was released");
+    e->commits = ctx->commits;
+  }
+  return HFB_OK;
+}
+// at least n_a free slots in front of B in the env's table; B moves (device to device) when the table regrows
+static int env_make_room(hfb_ctx* ctx, hfb_env* e, size_t n_a, cudaStream_t s) {
+  if (n_a <= e->head) return HFB_OK;
+  const size_t head = n_a + n_a / 4;
+  DevBuf h, tf;
+  cudaError_t err = h.reserve((head + e->n_b) * 4);
+  if (err == cudaSuccess) err = tf.reserve((head + e->n_b) * sizeof(hfb_transform));
+  if (err == cudaSuccess)
+    err = cudaMemcpyAsync(static_cast<uint32_t*>(h.p) + head, static_cast<uint32_t*>(e->h.p) + e->head, e->n_b * 4,
+                          cudaMemcpyDeviceToDevice, s);
+  if (err == cudaSuccess)
+    err = cudaMemcpyAsync(static_cast<hfb_transform*>(tf.p) + head, static_cast<hfb_transform*>(e->tf.p) + e->head,
+                          e->n_b * sizeof(hfb_transform), cudaMemcpyDeviceToDevice, s);
+  if (err == cudaSuccess) err = cudaStreamSynchronize(s);
+  if (err != cudaSuccess) {
+    h.release();
+    tf.release();
+    return cuda_fail(ctx, err, "environment table");
+  }
+  e->h.release();
+  e->tf.release();
+  e->h = h;
+  e->tf = tf;
+  e->head = head;
+  return HFB_OK;
+}
+// the cross grid over B's boxes (scratch: the context's bp_scratch)
+static int env_build(hfb_ctx* ctx, hfb_env* e, cudaStream_t s) {
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(0, e->n_b)));
+  int nl = 0;
+  if (bp_cross_build_launch(e->n_b, static_cast<const double*>(e->bb.p), bp_cross_grid_carve(e->grid.p, e->n_b),
+                            ctx->bp_scratch.p, s, &nl) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "cross grid launch failed");
+  ctx->stats.kernel_launches += (uint64_t)nl;
+  return HFB_OK;
+}
+// one query of A (already in the table in front of B) against the env: boxes of A, the candidates against the built
+// grid, the narrow phase, then the outputs (host or device)
+static int env_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a, const hfb_collision_request* req,
+                     bool minus_inf, const hfb_env_out* out, cudaStream_t s, bool dev) {
+  const size_t n_b = e->n_b, a_hi = first_a + (num_a < n_a ? num_a : n_a);
+  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+  const double* bb_b = static_cast<const double*>(e->bb.p);
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+    if (int rc = bp_cross_query_reset(g, d_cnt, s)) return rc;
+    return bp_cross_query_launch(n_a, d_bb, first_a, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt, ctx->bp_scratch.p,
+                                 ctx->num_sms, s, nl);
+  };
+  const size_t off = e->head - n_a;
+  unsigned cand = 0;
+  if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
+                                static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand))
+    return rc;
+  if (out->n_candidates) {
+    if (dev)
+      CK(cudaMemcpyAsync(out->n_candidates, ctx->sc_cnt.p, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
+    else
+      *out->n_candidates = cand;
+  }
+  if (cand == 0 || minus_inf) return HFB_OK;
+  return scene_output(ctx, s, cand, (uint32_t)n_a, out, n_a, dev);
+}
+
+extern "C" {
+
+int hfb_env_create(hfb_ctx* ctx, size_t n_b, const uint32_t* handles_b, const hfb_transform* tfs_b, hfb_env** out) {
+  if (!ctx || !out || (n_b && (!handles_b || !tfs_b))) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = check_ready(ctx)) return rc;
+  if (n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = check_handles(ctx, handles_b, n_b)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  std::unique_ptr<hfb_env> e(new hfb_env);
+  e->n_b = n_b;
+  e->handles.assign(handles_b, handles_b + n_b);
+  e->commits = ctx->commits;
+  e->clears = ctx->clears;
+  CK(e->h.reserve(n_b * 4 + 4));
+  CK(e->tf.reserve(n_b * sizeof(hfb_transform) + 8));
+  CK(e->bb.reserve(n_b * 48 + 8));
+  CK(e->grid.reserve(bp_cross_grid_bytes(n_b)));
+  if (n_b) {
+    CK(cudaMemcpyAsync(e->h.p, handles_b, n_b * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(e->tf.p, tfs_b, n_b * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+    if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n_b, static_cast<const uint32_t*>(e->h.p),
+                              static_cast<const hfb_transform*>(e->tf.p), static_cast<double*>(e->bb.p), s) != 0)
+      return fail(ctx, HFB_ERR_CUDA, "k_scene_aabbs launch failed");
+    ctx->stats.kernel_launches++;
+  }
+  if (int rc = env_build(ctx, e.get(), s)) return rc;
+  CK(cudaStreamSynchronize(s));
+  ctx->envs.push_back(e.get());
+  *out = e.release();
+  return HFB_OK;
+}
+
+int hfb_env_update(hfb_ctx* ctx, hfb_env* env, size_t m, const uint32_t* indices, const hfb_transform* tfs) {
+  if (!ctx || !env || (m && (!indices || !tfs))) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = env_ready(ctx, env)) return rc;
+  std::vector<uint8_t> seen(m ? env->n_b : 0, 0);  // all or nothing: every index checked before anything moves
+  for (size_t k = 0; k < m; ++k) {
+    if (indices[k] >= env->n_b) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "environment index out of range");
+    if (seen[indices[k]]++) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "environment index repeated");
+  }
+  if (m == 0) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  CK(ctx->obj_h.reserve(m * 4 + 4));
+  CK(ctx->obj_tf.reserve(m * sizeof(hfb_transform) + 8));
+  CK(cudaMemcpyAsync(ctx->obj_h.p, indices, m * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(ctx->obj_tf.p, tfs, m * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  if (bp_env_update_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, m, static_cast<const uint32_t*>(ctx->obj_h.p),
+                           static_cast<const hfb_transform*>(ctx->obj_tf.p), static_cast<const uint32_t*>(env->h.p) + env->head,
+                           static_cast<hfb_transform*>(env->tf.p) + env->head, static_cast<double*>(env->bb.p), s) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "k_env_update launch failed");
+  ctx->stats.kernel_launches++;
+  if (int rc = env_build(ctx, env, s)) return rc;
+  CK(cudaStreamSynchronize(s));
+  return HFB_OK;
+}
+
+int hfb_env_collide(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                    size_t first_a, size_t num_a, const hfb_collision_request* req, const hfb_env_out* out) {
+  if (!ctx || !env || !req || !out || (n_a && (!handles_a || !tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
+  if (out->capacity && (!out->first || !out->second || !out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
+  if (out->n_candidates) *out->n_candidates = 0;
+  if (out->n_colliding) *out->n_colliding = 0;
+  if (out->flags && n_a) std::memset(out->flags, 0, n_a);
+  if (n_a == 0 || env->n_b == 0) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+  const size_t off = env->head - n_a;
+  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  return env_query(ctx, env, n_a, first_a, num_a, req, minus_inf, out, s, false);
+}
+
+int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a, const hfb_transform* d_tfs_a,
+                           size_t first_a, size_t num_a, const hfb_collision_request* req, const hfb_env_out* d_out,
+                           void* stream) {
+  if (!ctx || !env || !req || !d_out || (n_a && (!d_handles_a || !d_tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
+  if (d_out->capacity && (!d_out->first || !d_out->second || !d_out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (d_out->n_candidates) CK(cudaMemsetAsync(d_out->n_candidates, 0, sizeof(uint32_t), s));
+  if (d_out->n_colliding) CK(cudaMemsetAsync(d_out->n_colliding, 0, sizeof(uint32_t), s));
+  if (d_out->flags && n_a) CK(cudaMemsetAsync(d_out->flags, 0, n_a, s));
+  if (n_a && env->n_b) {
+    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+    const size_t off = env->head - n_a;
+    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
+                       cudaMemcpyDeviceToDevice, s));
+    if (int rc = env_query(ctx, env, n_a, first_a, num_a, req, minus_inf, d_out, s, true)) return rc;
+  }
+  // the next call that shares the scratch or this table waits for what is still running here
+  CK(cudaEventRecord(ctx->dev_done, s));
+  ctx->dev_used = true;
+  ctx->dev_last_stream = s;
+  return HFB_OK;
+}
+
+int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env) {
+  if (!ctx || !env) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  auto it = std::find(ctx->envs.begin(), ctx->envs.end(), env);
+  if (it == ctx->envs.end()) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "not an environment of this context");
+  CK(cudaSetDevice(ctx->device));
+  // what may still read its table: the last device query (each one waits for the one before on another stream) and
+  // the host calls' stream
+  if (ctx->dev_used) CK(cudaEventSynchronize(ctx->dev_done));
+  CK(cudaStreamSynchronize(ctx->slots[0].stream));
+  ctx->envs.erase(it);
+  delete env;
+  return HFB_OK;
 }
 
 int hfb_batch_convex_support_device(hfb_ctx* ctx, size_t n, const uint32_t* ids, const double* dirs,

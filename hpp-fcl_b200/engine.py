@@ -66,6 +66,11 @@ def load_library(path=None):
     L.hfb_broadphase_cross_pairs.argtypes = [sz, vp, sz, vp, vp, vp, sz, vp]
     L.hfb_broadphase_cross_pairs_device.argtypes = [vp, sz, vp, sz, sz, sz, vp, vp, vp, sz, vp, vp]
     L.hfb_scene_collide_sets.argtypes = [vp, sz, vp, vp, sz, vp, vp, sz, sz, vp, vp]
+    L.hfb_env_create.argtypes = [vp, sz, vp, vp, C.POINTER(vp)]
+    L.hfb_env_update.argtypes = [vp, vp, sz, vp, vp]
+    L.hfb_env_collide.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, vp]
+    L.hfb_env_collide_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, vp, vp]
+    L.hfb_env_destroy.argtypes = [vp, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -384,6 +389,60 @@ class Engine:
                                                   na if num_a is None else num_a, C.byref(req), C.byref(out)))
         k = min(int(nc[0]), cap)
         return f[:k], s2[:k], rec[:k], int(nc[1]), int(nc[0])
+
+    # -- resident environment (hfb_env_*): set B's table, boxes and grid kept on the device across queries -------
+    def env_create(self, handles_b, tfs_b):
+        """set B on the device (its boxes as of now and the cross grid over them) -> an opaque env handle"""
+        hb = np.ascontiguousarray(handles_b, dtype=np.uint32)
+        tb = np.ascontiguousarray(tfs_b, dtype=P.transform_dtype)
+        if hb.shape[0] != tb.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        env = C.c_void_p()
+        self._check(self.L.hfb_env_create(self.h, hb.shape[0], _ptr(hb), _ptr(tb), C.byref(env)))
+        return env
+
+    def env_update(self, env, indices, tfs):
+        """new poses of the B objects `indices` (the reference's update(objs)); their boxes and the grid are redone"""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32)
+        t = np.ascontiguousarray(tfs, dtype=P.transform_dtype)
+        if idx.shape[0] != t.shape[0]:
+            raise ValueError("index and pose arrays must have equal length")
+        self._check(self.L.hfb_env_update(self.h, env, idx.shape[0], _ptr(idx), _ptr(t)))
+
+    def env_collide(self, env, handles_a, tfs_a, req=None, capacity=None, first_a=0, num_a=None, flags=False, bufs=None):
+        """set A against the env (hfb_env_collide): what scene_collide_sets(A, B) returns -> (first = index in A, second =
+        index in B, contacts, n_candidates, n_colliding), plus one flag byte per A object (1: it collides) with
+        flags=True.  capacity=0 with flags=True: no pair records at all"""
+        req = req or P.CollisionRequestPOD()
+        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
+        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
+        if ha.shape[0] != ta.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        na = ha.shape[0]
+        cap = int(capacity) if capacity is not None else max(4 * na, 1024)
+        if bufs is None:
+            bufs = (np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=np.uint32), np.empty(cap, dtype=P.contact_dtype))
+        f, s2, rec = bufs
+        fl = np.empty(na, dtype=np.uint8) if flags else None
+        nc = np.zeros(2, dtype=np.uint32)
+        out = P.EnvOut(f.ctypes.data, s2.ctypes.data, rec.ctypes.data, cap, nc[0:1].ctypes.data, nc[1:2].ctypes.data,
+                       None if fl is None else fl.ctypes.data)
+        self._check(self.L.hfb_env_collide(self.h, env, na, _ptr(ha), _ptr(ta), first_a, na if num_a is None else num_a,
+                                           C.byref(req), C.byref(out)))
+        k = min(int(nc[0]), cap)
+        res = (f[:k], s2[:k], rec[:k], int(nc[1]), int(nc[0]))
+        return res + (fl,) if flags else res
+
+    def env_collide_device(self, env, n_a, d_handles_a, d_tfs_a, d_first, d_second, d_contacts, capacity, d_n_colliding,
+                           d_n_candidates, d_flags=None, req=None, stream=0, first_a=0, num_a=None):
+        """hfb_env_collide_device: A's handles and poses and every output are device pointers, ordered on `stream`"""
+        req = req or P.CollisionRequestPOD()
+        out = P.EnvOut(d_first, d_second, d_contacts, capacity, d_n_colliding, d_n_candidates, d_flags)
+        self._check(self.L.hfb_env_collide_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a), first_a,
+                                                  n_a if num_a is None else num_a, C.byref(req), C.byref(out), _ptr(stream)))
+
+    def env_destroy(self, env):
+        self._check(self.L.hfb_env_destroy(self.h, env))
 
     # -- object-table queries: the batched form of the CollisionObject overloads (collision.h:58-61) -----
     @staticmethod

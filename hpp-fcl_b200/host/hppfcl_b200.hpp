@@ -729,6 +729,30 @@ class DynamicAABBTreeCollisionManager {
   void getObjects(std::vector<CollisionObject*>& out) const { out = objs; }
   void setup() { refresh(); }
   void update() { refresh(); }
+  /// the box of one object / of some objects from their current poses (broadphase_collision_manager.h:76-79)
+  void update(CollisionObject* updated_obj) { update(std::vector<CollisionObject*>(1, updated_obj)); }
+  void update(const std::vector<CollisionObject*>& updated_objs) {
+    if (stale) return refresh();
+    std::vector<size_t> idx;
+    std::vector<uint32_t> h;
+    std::vector<hfb_transform> t;
+    for (CollisionObject* o : updated_objs) {
+      const size_t i = std::find(objs.begin(), objs.end(), o) - objs.begin();
+      if (i == objs.size()) continue;  // not one of this manager's objects
+      tfs[i] = o->getTransform().pod();
+      idx.push_back(i);
+      h.push_back(hs[i]);
+      t.push_back(tfs[i]);
+    }
+    std::vector<double> bb(6 * idx.size());
+    C.check(hfb_scene_aabbs(C.raw(), idx.size(), h.data(), t.data(), bb.data()));
+    for (size_t k = 0; k < idx.size(); ++k) {
+      std::copy(bb.begin() + 6 * k, bb.begin() + 6 * k + 6, boxes.begin() + 6 * idx[k]);
+      AABB& b = objs[idx[k]]->getAABB();
+      b.min_ = Vec3f(bb[6 * k], bb[6 * k + 1], bb[6 * k + 2]);
+      b.max_ = Vec3f(bb[6 * k + 3], bb[6 * k + 4], bb[6 * k + 5]);
+    }
+  }
   /// self collision: callback(o1, o2) for every pair with overlapping boxes until it returns true
   void collide(CollisionCallBackBase* callback) {
     callback->init();
@@ -795,6 +819,7 @@ class DynamicAABBTreeCollisionManager {
   Context& context() { return C; }
 
  private:
+  friend class ResidentEnvironment;
   void cross_pairs(const double* boxes_b, size_t n_b, std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
     size_t cap = std::max<size_t>(16 * (objs.size() + n_b), 1024), cnt = 0;
     for (;;) {
@@ -882,6 +907,74 @@ inline std::vector<hfb_contact> collide(DynamicAABBTreeCollisionManager& manager
   manager.context().check(hfb_batch_collide_objects(manager.context().raw(), &sc, &q, out.data(), nullptr, nullptr));
   return out;
 }
+
+/// A manager's objects kept on the device as set B of the two-set collide (hfb_env): the table, the boxes as of
+/// construction / update(objs) and the grid over them stay there between queries, as the reference's tree does between
+/// setup() and update().  collide() and collide_flags() upload only the robot manager's poses.  Owns the hfb_env.
+class ResidentEnvironment {
+ public:
+  explicit ResidentEnvironment(DynamicAABBTreeCollisionManager& manager) : C(manager.C) {
+    if (manager.stale) manager.refresh();
+    for (size_t i = 0; i < manager.objs.size(); ++i) index[manager.objs[i]] = (uint32_t)i;
+    C.check(hfb_env_create(C.raw(), manager.hs.size(), manager.hs.data(), manager.tfs.data(), &env));
+  }
+  ~ResidentEnvironment() { hfb_env_destroy(C.raw(), env); }
+  ResidentEnvironment(const ResidentEnvironment&) = delete;
+  ResidentEnvironment& operator=(const ResidentEnvironment&) = delete;
+  /// the current poses of these environment objects pushed to the device (their boxes and the grid are redone)
+  void update(const std::vector<CollisionObject*>& objs) {
+    std::vector<uint32_t> idx;
+    std::vector<hfb_transform> t;
+    for (CollisionObject* o : objs) {
+      auto it = index.find(o);
+      if (it == index.end()) throw std::invalid_argument("not an object of this environment");
+      idx.push_back(it->second);
+      t.push_back(o->getTransform().pod());
+    }
+    C.check(hfb_env_update(C.raw(), env, idx.size(), idx.data(), t.data()));
+  }
+  /// the colliding pairs (first: index in the robot manager, second: index in the environment) and their records
+  std::vector<hfb_contact> collide(DynamicAABBTreeCollisionManager& robot, const CollisionRequest& request,
+                                   std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    uint32_t hits = 0, cand = 0;
+    std::vector<hfb_contact> rec;
+    for (size_t cap = std::max<size_t>(4 * robot.hs.size(), 1024);;) {
+      first.resize(cap);
+      second.resize(cap);
+      rec.resize(cap);
+      hfb_env_out out{first.data(), second.data(), rec.data(), (uint32_t)cap, &hits, &cand, nullptr};
+      C.check(hfb_env_collide(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), 0, robot.hs.size(), &q, &out));
+      if (hits <= cap) break;
+      cap = hits;
+    }
+    first.resize(hits);
+    second.resize(hits);
+    rec.resize(hits);
+    return rec;
+  }
+  /// one byte per robot object: 1 iff it collides with the environment (no pair records come back)
+  std::vector<uint8_t> collide_flags(DynamicAABBTreeCollisionManager& robot, const CollisionRequest& request) {
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    std::vector<uint8_t> flags(robot.hs.size());
+    hfb_env_out out{nullptr, nullptr, nullptr, 0, nullptr, nullptr, flags.data()};
+    C.check(hfb_env_collide(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), 0, robot.hs.size(), &q, &out));
+    return flags;
+  }
+
+ private:
+  void prepare(DynamicAABBTreeCollisionManager& robot, const CollisionRequest& request, hfb_collision_request& q) {
+    if (request.num_max_contacts == 0 && request.security_margin != -std::numeric_limits<FCL_REAL>::infinity())
+      throw std::invalid_argument("Invalid number of max contacts (current value is 0).");
+    if (robot.stale) robot.refresh();
+    detail::fill(request, q);
+  }
+  Context& C;
+  hfb_env* env = nullptr;
+  std::unordered_map<const CollisionObject*, uint32_t> index;
+};
 
 // ---------------------------------------------------------------- free functions
 // collide(): src/collision.cpp:69-130 (results accumulate; callers clear()).

@@ -438,6 +438,46 @@ int hfb_scene_collide_sets(hfb_ctx* ctx, size_t n_a, const uint32_t* handles_a, 
                            const uint32_t* handles_b, const hfb_transform* tfs_b, size_t first_a, size_t num_a,
                            const hfb_collision_request* req, const hfb_scene_contacts* out);
 
+/* ---- resident environment: set B kept on the device across hfb_scene_collide_sets-style queries -----------------
+ * The reference's managers are set up once and queried many times (DynamicAABBTreeCollisionManager::setup(), then
+ * update(obj) / update(objs) for the objects that moved: broadphase_dynamic_AABB_tree.cpp:587-647).  An hfb_env holds
+ * set B's object table, its boxes and the cross grid over them on the device, so a query uploads only A.  B's boxes are
+ * a snapshot taken at create / update time, as the reference's tree is; the narrow phase uses the current geometry
+ * and B's stored poses.
+ *   hfb_env_create:  HOST buffers; B's handles are validated as hfb_scene_collide_sets validates them.
+ *   hfb_env_update:  new poses of m objects of B (indices into B, HOST buffers): the reference's update(objs).  An index
+ *                    out of range or repeated is HFB_ERR_INVALID_ARGUMENT and changes nothing.
+ *   hfb_env_collide: HOST buffers, blocking.  What hfb_scene_collide_sets(A, B) returns for the same inputs (o1 from A,
+ *                    o2 from B, the same counts, [first_a, first_a + num_a) the same way).
+ *   hfb_env_collide_device: A's handles and poses and every output in DEVICE memory, ordered on `cuda_stream`; the
+ *                    call blocks once, for the candidate count that sizes the narrow phase, and once more, on
+ *                    `cuda_stream`, when A has more objects than any query before and the env's table regrows.
+ *   hfb_env_destroy: frees it; hfb_ctx_destroy frees the envs a context still owns.
+ * After a later hfb_geom_commit, B's handles are checked again before the next query: a handle released since is
+ * HFB_ERR_INVALID_ARGUMENT.  After hfb_geom_clear every env of the context is refused until it is destroyed. */
+typedef struct hfb_env hfb_env;
+/* hfb_scene_contacts plus `flags` (may be null): flags[i] = 1 iff A object i has at least one colliding candidate pair,
+ * for all n_a objects (0 outside [first_a, first_a + num_a)) -- the batched verdict CollisionCallBackDefault leaves in
+ * data.result.isCollision() (default_broadphase_callbacks.cpp:43-60).  With flags set and capacity == 0 no pair records
+ * are compacted or downloaded; the counts are still written. */
+typedef struct hfb_env_out {
+  uint32_t* first;
+  uint32_t* second;
+  hfb_contact* contacts;
+  uint32_t capacity;
+  uint32_t* n_colliding;
+  uint32_t* n_candidates;
+  uint8_t* flags;
+} hfb_env_out;
+int hfb_env_create(hfb_ctx* ctx, size_t n_b, const uint32_t* handles_b, const hfb_transform* tfs_b, hfb_env** out);
+int hfb_env_update(hfb_ctx* ctx, hfb_env* env, size_t m, const uint32_t* indices, const hfb_transform* tfs);
+int hfb_env_collide(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                    size_t first_a, size_t num_a, const hfb_collision_request* req, const hfb_env_out* out);
+int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                           const hfb_transform* d_tfs_a, size_t first_a, size_t num_a, const hfb_collision_request* req,
+                           const hfb_env_out* d_out, void* cuda_stream);
+int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
