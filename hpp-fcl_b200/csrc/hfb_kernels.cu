@@ -856,7 +856,7 @@ struct hfb_ctx {
   int bvh_quorum = HFB_BVH_INIT_QUORUM;  // HFB_BVH_QUORUM=1: a lane sets its next query up as soon as it is free
   int bvh_order = 0;  // HFB_BVH_ORDER=1: hand the (mesh, shape) queries out longest-expected first
   int bvhq = 1;        // HFB_BVHQ=0: mesh-shape distance queries through the lane-per-query kernel k_bvh instead of the task system k_bvhq
-  // HFB_GJK_PASSES="6" (default) or e.g. "3,3,4": iterations of the first passes of the primitive-pair GJK (one more pass runs to
+  // HFB_GJK_PASSES="10" (default) or e.g. "3,3,4": iterations of the first passes of the primitive-pair GJK (one more pass runs to
   // convergence); "0": the single kernel k_pairs<1, CAP_PRIM, MODE, PATH_GJKROUTE>
   // iterations of the first pass: 10 (a pass of few iterations leaves most pairs to the next; a long one idles the lanes
   // of the pairs that converged early)
