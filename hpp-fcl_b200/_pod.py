@@ -158,6 +158,10 @@ class EnvOut(C.Structure):  # hfb_env_out: hfb_scene_contacts + one flag byte pe
     _fields_ = SceneContacts._fields_ + [("flags", C.c_void_p)]
 
 
+class ConfigsOut(C.Structure):  # hfb_configs_out: one verdict byte per configuration, the two kinds of pairs
+    _fields_ = [("verdicts", C.c_void_p), ("env", SceneContacts), ("self", SceneContacts)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -703,6 +703,25 @@ class ResidentEnvironment:
         h, t, req = self._robot(robot_manager, request)
         return self.engine.env_collide(self._env, h, t, req, capacity=0, flags=True)[5]
 
+    def collide_configurations(self, robot_manager, links_per_config, self_pairs, request=None, capacity=None):
+        """A planner's validity check: the robot manager holds configurations of links_per_config objects each,
+        configuration-major (object g * L + i is link i of configuration g); self_pairs is the template of link pairs
+        (i, j) each configuration checks against itself (an SRDF's enabled pairs).  -> (verdicts: one byte per
+        configuration, 1 iff it collides with the environment or with itself; environment pairs (first = index in the
+        robot manager, second = index in the environment, contact records); self pairs (first, second: indices in the
+        robot manager, contact records)), the pairs in no particular order"""
+        h, t, req = self._robot(robot_manager, request)
+        v, e, s = self.engine.env_collide_configs(self._env, h, t, links_per_config, self_pairs, req, capacity, capacity)
+        if capacity is None and (e[4] > len(e[0]) or s[4] > len(s[0])):  # (all of them unless a capacity is given)
+            v, e, s = self.engine.env_collide_configs(self._env, h, t, links_per_config, self_pairs, req, e[4], s[4])
+        return v, e[:3], s[:3]
+
+    def configuration_flags(self, robot_manager, links_per_config, self_pairs, request=None):
+        """-> one byte per configuration: 1 iff it collides with the environment or with itself (no pair records come
+        back)"""
+        h, t, req = self._robot(robot_manager, request)
+        return self.engine.env_collide_configs(self._env, h, t, links_per_config, self_pairs, req, 0, 0)[0]
+
     def close(self):
         if getattr(self, "_env", None) is not None and getattr(self.engine, "h", None):
             self.engine.env_destroy(self._env)

@@ -405,6 +405,20 @@ __global__ void __launch_bounds__(128) k_cross_oversize(const double* ba, unsign
   }
 }
 
+// the self pairs of configurations [g0, g0 + total / P) (config_pair): one thread per (configuration, template pair),
+// appended to the same counter as whatever ran before on it
+__global__ void __launch_bounds__(128) k_config_pairs(const double* bb, unsigned links, const uint32_t* tpl, unsigned n_tpl,
+                                                      unsigned g0, size_t total, uint32_t* first, uint32_t* second,
+                                                      unsigned capacity, unsigned* n_pairs) {
+  const size_t tend = (total + 31u) & ~(size_t)31;  // (warp-uniform trip count for the ballots)
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < tend; t += (size_t)gridDim.x * blockDim.x) {
+    bool hit = false;
+    uint32_t a = 0, b = 0;
+    if (t < total) hit = config_pair(bb, links, tpl, n_tpl, g0, t, &a, &b);
+    append_pair(hit, a, b, first, second, capacity, n_pairs);
+  }
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -616,6 +630,21 @@ int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size
   if (int e = cross_grid_bin(n_b, d_aabbs_b, g, scratch, s, launches)) return e;
   return cross_sweep(a_lo, a_hi, d_aabbs_a, n_b, d_aabbs_b, g, g.counters, d_first, d_second, second_base,
                      (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity), d_n_pairs, scratch, num_sms, s, launches);
+}
+
+int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
+                           size_t num_configs, uint32_t* d_first, uint32_t* d_second, size_t capacity, unsigned* d_n_pairs,
+                           int num_sms, cudaStream_t s, int* launches) {
+  const size_t total = num_configs * n_tpl;
+  if (total == 0) return 0;
+  if (num_sms < 1) num_sms = 1;
+  size_t nb = (total + 127) / 128;
+  if (nb > (size_t)num_sms * 16u) nb = (size_t)num_sms * 16u;
+  k_config_pairs<<<(unsigned)nb, 128, 0, s>>>(d_aabbs, (unsigned)links, d_tpl, (unsigned)n_tpl, (unsigned)g0, total, d_first,
+                                              d_second, (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity),
+                                              d_n_pairs);
+  *launches += 1;
+  return (int)cudaGetLastError();
 }
 
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,

@@ -415,4 +415,54 @@ inline size_t broadphase_cross_pairs_host(size_t na, const double* ba, size_t nb
   return count;
 }
 
+// ---- self pairs within configurations: a robot checked against itself, one configuration at a time ----------------
+// Set A holds configurations of L links each, configuration-major (object g*L + i is link i of configuration g).  A
+// template of P link pairs (i, j) -- an SRDF's enabled pairs, the collision pairs of a Pinocchio GeometryModel -- names
+// the pairs each configuration checks.  The candidates of configuration g are the template's pairs whose boxes
+// overlap: the set DynamicAABBTreeCollisionManager::collide(callback) over g's L objects hands to a callback that keeps
+// only the template's pairs (broadphase_collision_manager.h:104-106), with o1 = g*L + i and o2 = g*L + j.  No grid: a
+// configuration has a few hundred pairs at most, each a test of two boxes.
+
+// the template's conditions; null when it meets them
+inline const char* config_template_error(size_t links, size_t n_pairs, const uint32_t* tpl) {
+  std::vector<uint64_t> keys(n_pairs);
+  for (size_t k = 0; k < n_pairs; ++k) {
+    const uint32_t i = tpl[2 * k], j = tpl[2 * k + 1];
+    if (i >= links || j >= links) return "self-pair template: link index out of range";
+    if (i == j) return "self-pair template: a link paired with itself";
+    keys[k] = i < j ? (uint64_t)i << 32 | j : (uint64_t)j << 32 | i;
+  }
+  std::sort(keys.begin(), keys.end());
+  if (std::adjacent_find(keys.begin(), keys.end()) != keys.end()) return "self-pair template: a pair listed twice";
+  return nullptr;
+}
+// self pair t of the configurations from g0 on: configuration g0 + t / P, template entry t % P -> (*a, *b), object
+// indices in A; true when both objects have a box and the boxes overlap (AABB::overlap, closed intervals)
+HFB_HD bool config_pair(const double* bb, uint32_t links, const uint32_t* tpl, uint32_t n_pairs, uint32_t g0, size_t t,
+                        uint32_t* a, uint32_t* b) {
+  const size_t g = g0 + t / n_pairs, k = t % n_pairs;
+  *a = (uint32_t)(g * links + tpl[2 * k]);
+  *b = (uint32_t)(g * links + tpl[2 * k + 1]);
+  const double* x = bb + 6 * (size_t)*a;
+  const double* y = bb + 6 * (size_t)*b;
+  return !aabb_empty(x) && !aabb_empty(y) && aabb_overlap(x, y);
+}
+// the self pairs of configurations [g0, g0 + num_configs), configuration by configuration in template order; returns
+// their number (all of them are counted, at most `capacity` stored)
+inline size_t broadphase_config_pairs_host(const double* bb, uint32_t links, const uint32_t* tpl, uint32_t n_pairs,
+                                           uint32_t g0, size_t num_configs, uint32_t* first, uint32_t* second,
+                                           size_t capacity) {
+  size_t count = 0;
+  for (size_t t = 0; t < num_configs * n_pairs; ++t) {
+    uint32_t a, b;
+    if (!config_pair(bb, links, tpl, n_pairs, g0, t, &a, &b)) continue;
+    if (count < capacity) {
+      first[count] = a;
+      second[count] = b;
+    }
+    ++count;
+  }
+  return count;
+}
+
 }  // namespace hfb

@@ -48,6 +48,13 @@ int bp_cross_query_reset(const BpCrossGrid& g, unsigned* d_n_pairs, cudaStream_t
 int bp_cross_query_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size_t a_hi, size_t n_b, const double* d_aabbs_b,
                           const BpCrossGrid& g, uint32_t* d_first, uint32_t* d_second, uint32_t second_base, size_t capacity,
                           unsigned* d_n_pairs, void* scratch, int num_sms, cudaStream_t s, int* launches);
+// the self pairs of configurations [g0, g0 + num_configs) of L = `links` objects each (config_pair of
+// hfb_broadphase.cuh; d_tpl: n_tpl pairs of link indices, validated) -> (d_first, d_second), APPENDED after the pairs
+// *d_n_pairs already counts; at most `capacity` stored in all.  Returns a cudaError_t as int; *launches += kernels
+// launched.
+int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
+                           size_t num_configs, uint32_t* d_first, uint32_t* d_second, size_t capacity, unsigned* d_n_pairs,
+                           int num_sms, cudaStream_t s, int* launches);
 // hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
                          const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,

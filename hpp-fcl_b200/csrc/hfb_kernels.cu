@@ -715,6 +715,21 @@ __global__ void __launch_bounds__(256) k_unbase(uint32_t* second, const unsigned
   const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < *count && i < cap) second[i] -= base;
 }
+// hfb_env_collide_configs' verdicts: the configuration (A index / links) of a colliding candidate gets 1; when no
+// compaction counts them (counts null: not counted), counts[0] / counts[1] get the colliding candidates before / from
+// `split` on (environment pairs, self pairs)
+__global__ void __launch_bounds__(256) k_flag_configs(const hfb_contact* r, const uint32_t* pf, unsigned n, unsigned links,
+                                                      unsigned split, uint8_t* verdicts, unsigned* counts) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool hit = i < n && r[i].num_contacts > 0;
+  if (hit) verdicts[pf[i] / links] = 1;
+  if (!counts) return;
+  const unsigned me = __ballot_sync(0xffffffffu, hit && i < split), ms = __ballot_sync(0xffffffffu, hit && i >= split);
+  if ((threadIdx.x & 31u) == 0) {
+    if (me) atomicAdd(counts, (unsigned)__popc(me));
+    if (ms) atomicAdd(counts + 1, (unsigned)__popc(ms));
+  }
+}
 
 // ----------------------------------------------------- convex support kernel --
 // One warp per query: streams the SoA vertex block (coalesced 256-B rows) and
@@ -891,6 +906,7 @@ struct hfb_ctx {
   DevBuf bp_scratch;                // device broadphase
   DevBuf sc_bb, sc_pf, sc_ps, sc_cnt, sc_out, sc_f, sc_s, sc_rec;  // hfb_scene_collide
   DevBuf sc_flags;                                                 // hfb_env_collide
+  DevBuf sc_tpl;                                                   // hfb_env_collide_configs: the self-pair template
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   uint64_t commits = 0, clears = 0;
@@ -2467,10 +2483,11 @@ static int after_device_calls(hfb_ctx* ctx, cudaStream_t s) {
 // (d_h, d_tf: n objects): the boxes of its first n_boxes objects, the candidates (find_pairs(d_bb, pf, ps, capacity,
 // d_count, &launches) launches a pair finder, all pairs counted in *d_count, at most `capacity` stored) and collide() of
 // every candidate over the table, into ctx->sc_out (none when there are no candidates or under minus_inf).
+// split_out (may be null): the counter's second word, which a finder may set, read with the count.
 template <class FindPairs>
 static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
                             size_t n_boxes, FindPairs find_pairs, const hfb_collision_request* req, bool minus_inf,
-                            unsigned* cand_out) {
+                            unsigned* cand_out, unsigned* split_out = nullptr) {
   CK(ctx->sc_bb.reserve(n_boxes * 48));
   CK(ctx->sc_cnt.reserve(16));
   double* d_bb = static_cast<double*>(ctx->sc_bb.p);
@@ -2481,14 +2498,16 @@ static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32
   // the number of candidate pairs is not known in advance: a first sweep counts, a second one (if the buffers were too
   // small) stores
   size_t cap = ctx->sc_pf.cap / 4 < ctx->sc_ps.cap / 4 ? ctx->sc_pf.cap / 4 : ctx->sc_ps.cap / 4;
-  unsigned cand = 0;
+  unsigned cand = 0, words[2] = {0, 0};
   for (int attempt = 0; attempt < 2; ++attempt) {
     int nl = 0;
     if (find_pairs(d_bb, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p), cap, d_cnt, &nl) != 0)
       return fail(ctx, HFB_ERR_CUDA, "broadphase launch failed");
     ctx->stats.kernel_launches += (uint64_t)nl;
-    CK(cudaMemcpyAsync(&cand, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(words, d_cnt, (split_out ? 2 : 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
+    cand = words[0];
+    if (split_out) *split_out = words[1];
     if (cand <= cap) break;
     cap = (size_t)cand + cand / 8 + 1024;
     CK(ctx->sc_pf.reserve(cap * 4));
@@ -2630,6 +2649,23 @@ int hfb_broadphase_cross_pairs(size_t n_a, const double* aabbs_a, size_t n_b, co
       n_b > 0xffffffffull)
     return HFB_ERR_INVALID_ARGUMENT;
   *n_pairs = broadphase_cross_pairs_host(n_a, aabbs_a, n_b, aabbs_b, first, second, capacity);
+  return HFB_OK;
+}
+
+// the self candidates of configurations: collide(callback) over one configuration's objects with a callback that
+// keeps only the template's pairs (broadphase_collision_manager.h:104-106), for every configuration of the range
+int hfb_broadphase_config_pairs(size_t n_a, const double* aabbs, size_t links_per_config, size_t n_self_pairs,
+                                const uint32_t* self_pairs, size_t first_config, size_t num_configs, uint32_t* first,
+                                uint32_t* second, size_t capacity, size_t* n_pairs) {
+  if ((n_a && !aabbs) || !n_pairs || (capacity && (!first || !second)) || (n_self_pairs && !self_pairs) ||
+      n_a > 0xffffffffull || n_self_pairs > 0xffffffffull)
+    return HFB_ERR_INVALID_ARGUMENT;
+  const size_t L = links_per_config;
+  if (L == 0 || n_a % L || first_config > n_a / L || num_configs > n_a / L - first_config ||
+      config_template_error(L, n_self_pairs, self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  *n_pairs = broadphase_config_pairs_host(aabbs, (uint32_t)L, self_pairs, (uint32_t)n_self_pairs, (uint32_t)first_config,
+                                          num_configs, first, second, capacity);
   return HFB_OK;
 }
 
@@ -2775,6 +2811,130 @@ static int env_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_
   return scene_output(ctx, s, cand, (uint32_t)n_a, out, n_a, dev);
 }
 
+// hfb_env_collide_configs' arguments beyond the pointers: the layout of A, the configuration range and the template
+static int configs_args(hfb_ctx* ctx, size_t n_a, size_t links, size_t n_tpl, const uint32_t* tpl, size_t g0, size_t ng) {
+  if (links == 0 || n_a % links) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "n_a is not a multiple of links_per_config");
+  if (g0 > n_a / links || ng > n_a / links - g0) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "configuration range past the end");
+  if (n_tpl > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "self-pair template too large");
+  if (const char* e = config_template_error(links, n_tpl, tpl)) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, e);
+  return HFB_OK;
+}
+static bool contacts_ok(const hfb_scene_contacts& o) { return !o.capacity || (o.first && o.second && o.contacts); }
+
+// The outputs of hfb_env_collide_configs from the `cand` candidates, the environment pairs before `split`, the self
+// pairs from there on: verdicts per configuration, and each kind compacted into its own outputs with its own counter
+// (sc_cnt[1], sc_cnt[2]).  dev / host outputs as in scene_output.
+static int configs_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, unsigned split, uint32_t second_base, size_t links,
+                          size_t n_configs, const hfb_configs_out* out, bool dev) {
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+  const hfb_contact* recs = static_cast<const hfb_contact*>(ctx->sc_out.p);
+  const uint32_t* pf = static_cast<const uint32_t*>(ctx->sc_pf.p);
+  const uint32_t* ps = static_cast<const uint32_t*>(ctx->sc_ps.p);
+  const bool compact = !out->verdicts || out->env.capacity || out->self.capacity;
+  CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
+  uint8_t* verdicts = out->verdicts;
+  if (verdicts) {
+    if (!dev) {
+      CK(ctx->sc_flags.reserve(n_configs));
+      verdicts = static_cast<uint8_t*>(ctx->sc_flags.p);
+    }
+    CK(cudaMemsetAsync(verdicts, 0, n_configs, s));
+    k_flag_configs<<<(cand + 255) / 256, 256, 0, s>>>(recs, pf, cand, (unsigned)links, split, verdicts,
+                                                       compact ? nullptr : d_cnt + 1);
+    ctx->stats.kernel_launches++;
+  }
+  const hfb_scene_contacts* kinds[2] = {&out->env, &out->self};
+  const unsigned lo[2] = {0, split}, num[2] = {split, cand - split};
+  uint32_t *first[2], *second[2];
+  hfb_contact* contacts[2];
+  if (!dev) {  // both kinds staged in one set of buffers, the self pairs after the environment's
+    const size_t total = (size_t)out->env.capacity + out->self.capacity;
+    CK(ctx->sc_f.reserve(total * 4 + 4));
+    CK(ctx->sc_s.reserve(total * 4 + 4));
+    CK(ctx->sc_rec.reserve(total * sizeof(hfb_contact) + 8));
+  }
+  for (int k = 0; k < 2; ++k) {
+    const size_t at = k ? out->env.capacity : 0;
+    first[k] = dev ? kinds[k]->first : static_cast<uint32_t*>(ctx->sc_f.p) + at;
+    second[k] = dev ? kinds[k]->second : static_cast<uint32_t*>(ctx->sc_s.p) + at;
+    contacts[k] = dev ? kinds[k]->contacts : static_cast<hfb_contact*>(ctx->sc_rec.p) + at;
+    if (!compact || num[k] == 0) continue;
+    k_compact_scene<<<(num[k] + 255) / 256, 256, 0, s>>>(recs + lo[k], pf + lo[k], ps + lo[k], num[k], d_cnt + 1 + k,
+                                                          first[k], second[k], contacts[k], kinds[k]->capacity);
+    ctx->stats.kernel_launches++;
+  }
+  if (dev) {
+    const unsigned most = split < out->env.capacity ? split : out->env.capacity;
+    if (compact && most) {  // (only the environment's second indices are in B)
+      k_unbase<<<(most + 255) / 256, 256, 0, s>>>(out->env.second, d_cnt + 1, out->env.capacity, second_base);
+      ctx->stats.kernel_launches++;
+    }
+    for (int k = 0; k < 2; ++k)
+      if (kinds[k]->n_colliding)
+        CK(cudaMemcpyAsync(kinds[k]->n_colliding, d_cnt + 1 + k, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
+    CK(cudaGetLastError());
+    return HFB_OK;
+  }
+  unsigned hits[2] = {0, 0}, kept[2];
+  CK(cudaMemcpyAsync(hits, d_cnt + 1, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (int k = 0; k < 2; ++k) {
+    if (kinds[k]->n_colliding) *kinds[k]->n_colliding = hits[k];
+    kept[k] = !compact ? 0u : hits[k] < kinds[k]->capacity ? hits[k] : kinds[k]->capacity;
+    if (!kept[k]) continue;
+    CK(cudaMemcpyAsync(kinds[k]->first, first[k], (size_t)kept[k] * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(kinds[k]->second, second[k], (size_t)kept[k] * 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(kinds[k]->contacts, contacts[k], (size_t)kept[k] * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
+  }
+  if (verdicts) CK(cudaMemcpyAsync(out->verdicts, verdicts, n_configs, cudaMemcpyDeviceToHost, s));
+  if (kept[0] || kept[1] || verdicts) CK(cudaStreamSynchronize(s));
+  for (unsigned k = 0; k < kept[0]; ++k) out->env.second[k] -= second_base;
+  return HFB_OK;
+}
+
+// one configurations query of A (already in the table in front of B, the template in ctx->sc_tpl): one candidate
+// list -- the environment pairs against the built grid, then, after the split is noted in the counter's second word,
+// the self pairs appended to it -- one narrow phase over the table [A; B], then the outputs (host or device)
+static int env_configs_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t links, size_t n_tpl, size_t g0, size_t ng,
+                             const hfb_collision_request* req, bool minus_inf, const hfb_configs_out* out, cudaStream_t s,
+                             bool dev) {
+  const size_t n_b = e->n_b, a_lo = g0 * links, a_hi = (g0 + ng) * links;
+  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+  const double* bb_b = static_cast<const double*>(e->bb.p);
+  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+    int rc = 0;
+    if (n_b) {
+      rc = bp_cross_query_reset(g, d_cnt, s);
+      if (!rc)
+        rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt, ctx->bp_scratch.p,
+                                   ctx->num_sms, s, nl);
+    } else {
+      rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
+    }
+    if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
+    if (!rc) rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
+    return rc;
+  };
+  const size_t off = e->head - n_a;
+  unsigned cand = 0, split = 0;
+  if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
+                                static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand, &split))
+    return rc;
+  const unsigned n_cand[2] = {split, cand - split};
+  const hfb_scene_contacts* kinds[2] = {&out->env, &out->self};
+  for (int k = 0; k < 2; ++k) {
+    if (!kinds[k]->n_candidates) continue;
+    if (dev)  // (pageable source: staged before the call returns)
+      CK(cudaMemcpyAsync(kinds[k]->n_candidates, &n_cand[k], sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    else
+      *kinds[k]->n_candidates = n_cand[k];
+  }
+  if (cand == 0 || minus_inf) return HFB_OK;
+  return configs_output(ctx, s, cand, split, (uint32_t)n_a, links, n_a / links, out, dev);
+}
+
 extern "C" {
 
 int hfb_env_create(hfb_ctx* ctx, size_t n_b, const uint32_t* handles_b, const hfb_transform* tfs_b, hfb_env** out) {
@@ -2905,6 +3065,84 @@ int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env) {
   CK(cudaStreamSynchronize(ctx->slots[0].stream));
   ctx->envs.erase(it);
   delete env;
+  return HFB_OK;
+}
+
+// A planner's validity check in one call: every configuration of A against the env (hfb_env_collide's pairs) and
+// against itself (the template's link pairs per configuration), one verdict per configuration.  The reference asks
+// two queries per configuration: DynamicAABBTreeCollisionManager::collide(other_manager, callback) for the
+// environment (broadphase_collision_manager.h:94-118) and collide(callback) with a callback that keeps only the
+// template's pairs (:104-106), each with CollisionCallBackDefault (default_broadphase_callbacks.cpp:43-60).
+int hfb_env_collide_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_config,
+                            size_t num_configs, const hfb_collision_request* req, const hfb_configs_out* out) {
+  if (!ctx || !env || !req || !out || (n_a && (!handles_a || !tfs_a)) || (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  if (!contacts_ok(out->env) || !contacts_ok(out->self)) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
+  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
+  for (const hfb_scene_contacts* o : {&out->env, &out->self}) {
+    if (o->n_candidates) *o->n_candidates = 0;
+    if (o->n_colliding) *o->n_colliding = 0;
+  }
+  if (out->verdicts && n_a) std::memset(out->verdicts, 0, n_a / links_per_config);
+  if (n_a == 0 || num_configs == 0 || (env->n_b == 0 && n_self_pairs == 0)) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+  const size_t off = env->head - n_a;
+  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
+  if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
+  return env_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req, minus_inf, out, s,
+                           false);
+}
+
+int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                   const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                   const hfb_collision_request* req, const hfb_configs_out* d_out, void* stream) {
+  if (!ctx || !env || !req || !d_out || (n_a && (!d_handles_a || !d_tfs_a)) || (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  if (!contacts_ok(d_out->env) || !contacts_ok(d_out->self)) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  bool minus_inf;
+  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  for (const hfb_scene_contacts* o : {&d_out->env, &d_out->self}) {
+    if (o->n_candidates) CK(cudaMemsetAsync(o->n_candidates, 0, sizeof(uint32_t), s));
+    if (o->n_colliding) CK(cudaMemsetAsync(o->n_colliding, 0, sizeof(uint32_t), s));
+  }
+  if (d_out->verdicts && n_a) CK(cudaMemsetAsync(d_out->verdicts, 0, n_a / links_per_config, s));
+  if (n_a && num_configs && (env->n_b || n_self_pairs)) {
+    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+    const size_t off = env->head - n_a;
+    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
+                       cudaMemcpyDeviceToDevice, s));
+    CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
+    if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
+    if (int rc = env_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req, minus_inf,
+                                   d_out, s, true))
+      return rc;
+  }
+  // the next call that shares the scratch or this table waits for what is still running here
+  CK(cudaEventRecord(ctx->dev_done, s));
+  ctx->dev_used = true;
+  ctx->dev_last_stream = s;
   return HFB_OK;
 }
 

@@ -71,6 +71,9 @@ def load_library(path=None):
     L.hfb_env_collide.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, vp]
     L.hfb_env_collide_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, vp, vp]
     L.hfb_env_destroy.argtypes = [vp, vp]
+    L.hfb_env_collide_configs.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, vp]
+    L.hfb_env_collide_configs_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, vp, vp]
+    L.hfb_broadphase_config_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, vp, vp, sz, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -144,6 +147,34 @@ def broadphase_cross_pairs(aabbs_a, aabbs_b, capacity=None):
             k = min(cnt.value, cap)
             return first[:k], second[:k]
         cap = cnt.value
+
+
+def _template(self_pairs):
+    """a self-pair template as the C ABI takes it: (P, 2) uint32, contiguous"""
+    return np.ascontiguousarray(np.asarray(self_pairs, dtype=np.uint32).reshape(-1, 2))
+
+
+def broadphase_config_pairs(aabbs, links_per_config, self_pairs, first_config=0, num_configs=None, capacity=None):
+    """the self candidates of configurations: boxes (n x 6) of n_configs x links_per_config objects, configuration-major;
+    for every configuration g of [first_config, first_config + num_configs) (default: to the end) and template pair
+    (i, j) whose boxes overlap, (g * L + i, g * L + j) -> (first, second), configuration by configuration in template
+    order.  Host function of the library: needs neither a context nor a GPU."""
+    L = load_library()
+    bb = np.ascontiguousarray(aabbs, dtype=np.float64).reshape(-1, 6)
+    tpl = _template(self_pairs)
+    n, lpc = bb.shape[0], int(links_per_config)
+    if num_configs is None:
+        num_configs = max(n // lpc - first_config, 0) if lpc else 0
+    cap = int(capacity) if capacity is not None else max(tpl.shape[0] * int(num_configs), 1)
+    first = np.empty(max(cap, 1), dtype=np.uint32)
+    second = np.empty(max(cap, 1), dtype=np.uint32)
+    cnt = C.c_size_t(0)
+    rc = L.hfb_broadphase_config_pairs(n, _ptr(bb), lpc, tpl.shape[0], _ptr(tpl), int(first_config), int(num_configs),
+                                       _ptr(first), _ptr(second), cap, C.byref(cnt))
+    if rc != 0:
+        raise EngineError("hfb_broadphase_config_pairs: %s" % _ERR.get(rc, rc))
+    k = min(cnt.value, cap)
+    return first[:k], second[:k]
 
 
 def _ptr(a):
@@ -443,6 +474,52 @@ class Engine:
 
     def env_destroy(self, env):
         self._check(self.L.hfb_env_destroy(self.h, env))
+
+    def env_collide_configs(self, env, handles_a, tfs_a, links_per_config, self_pairs, req=None, env_capacity=None,
+                            self_capacity=None, first_config=0, num_configs=None, verdicts=True):
+        """configurations of links_per_config objects each (A, configuration-major) against the env and against
+        themselves (the template's link pairs), hfb_env_collide_configs -> (verdicts: one byte per configuration, 1 iff
+        it collides, or None with verdicts=False; env = (first = index in A, second = index in B, contacts, n_candidates,
+        n_colliding); self = (first, second: indices in A, contacts, n_candidates, n_colliding)).  Both capacities 0 with
+        verdicts=True: no pair records at all"""
+        req = req or P.CollisionRequestPOD()
+        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
+        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
+        if ha.shape[0] != ta.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        tpl = _template(self_pairs)
+        na, lpc = ha.shape[0], int(links_per_config)
+        n_configs = na // lpc if lpc else 0
+        caps = [int(c) if c is not None else max(4 * na, 1024) for c in (env_capacity, self_capacity)]
+        bufs = [(np.empty(c, dtype=np.uint32), np.empty(c, dtype=np.uint32), np.empty(c, dtype=P.contact_dtype)) for c in caps]
+        nc = np.zeros(4, dtype=np.uint32)  # env colliding, env candidates, self colliding, self candidates
+        v = np.empty(n_configs, dtype=np.uint8) if verdicts else None
+        kinds = [P.SceneContacts(f.ctypes.data, s2.ctypes.data, rec.ctypes.data, c, nc[2 * k:].ctypes.data,
+                                 nc[2 * k + 1:].ctypes.data) for k, ((f, s2, rec), c) in enumerate(zip(bufs, caps))]
+        out = P.ConfigsOut(None if v is None else v.ctypes.data, kinds[0], kinds[1])
+        self._check(self.L.hfb_env_collide_configs(self.h, env, na, _ptr(ha), _ptr(ta), lpc, tpl.shape[0], _ptr(tpl),
+                                                   first_config, n_configs - first_config if num_configs is None else num_configs,
+                                                   C.byref(req), C.byref(out)))
+        res = []
+        for k, ((f, s2, rec), c) in enumerate(zip(bufs, caps)):
+            m = min(int(nc[2 * k]), c)
+            res.append((f[:m], s2[:m], rec[:m], int(nc[2 * k + 1]), int(nc[2 * k])))
+        return v, res[0], res[1]
+
+    def env_collide_configs_device(self, env, n_a, d_handles_a, d_tfs_a, links_per_config, self_pairs, d_verdicts, env_out,
+                                   self_out, req=None, stream=0, first_config=0, num_configs=None):
+        """hfb_env_collide_configs_device: A's handles and poses and every output are device pointers, ordered on
+        `stream`; env_out / self_out = (d_first, d_second, d_contacts, capacity, d_n_colliding, d_n_candidates); the
+        template is a host array"""
+        req = req or P.CollisionRequestPOD()
+        tpl = _template(self_pairs)
+        lpc = int(links_per_config)
+        n_configs = n_a // lpc if lpc else 0
+        out = P.ConfigsOut(d_verdicts, P.SceneContacts(*env_out), P.SceneContacts(*self_out))
+        self._check(self.L.hfb_env_collide_configs_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a), lpc,
+                                                          tpl.shape[0], _ptr(tpl), first_config,
+                                                          n_configs - first_config if num_configs is None else num_configs,
+                                                          C.byref(req), C.byref(out), _ptr(stream)))
 
     # -- object-table queries: the batched form of the CollisionObject overloads (collision.h:58-61) -----
     @staticmethod

@@ -963,8 +963,72 @@ class ResidentEnvironment {
     C.check(hfb_env_collide(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), 0, robot.hs.size(), &q, &out));
     return flags;
   }
+  /// colliding pairs of one kind: object indices and the records
+  struct Pairs {
+    std::vector<uint32_t> first, second;
+    std::vector<hfb_contact> contacts;
+  };
+  /// A planner's validity check: the robot manager holds configurations of links_per_config objects each,
+  /// configuration-major (object g * L + i is link i of configuration g); self_pairs is the template of link pairs
+  /// (i, j) each configuration checks against itself (an SRDF's enabled pairs).  Returns one byte per configuration,
+  /// 1 iff it collides with the environment or with itself; env_pairs gets the colliding (robot index, environment
+  /// index) pairs, self_pairs_out the colliding (robot index, robot index) pairs.  A malformed template throws
+  /// std::invalid_argument.
+  std::vector<uint8_t> collide_configurations(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                              const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                              const CollisionRequest& request, Pairs& env_pairs, Pairs& self_pairs_out) {
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    std::vector<uint8_t> verdicts(links_per_config ? robot.hs.size() / links_per_config : 0);
+    uint32_t hits[2] = {0, 0}, cand[2] = {0, 0};
+    Pairs* kinds[2] = {&env_pairs, &self_pairs_out};
+    for (size_t cap[2] = {std::max<size_t>(4 * robot.hs.size(), 1024), std::max<size_t>(4 * robot.hs.size(), 1024)};;) {
+      hfb_scene_contacts o[2];
+      for (int k = 0; k < 2; ++k) {
+        kinds[k]->first.resize(cap[k]);
+        kinds[k]->second.resize(cap[k]);
+        kinds[k]->contacts.resize(cap[k]);
+        o[k] = {kinds[k]->first.data(), kinds[k]->second.data(), kinds[k]->contacts.data(), (uint32_t)cap[k], &hits[k], &cand[k]};
+      }
+      hfb_configs_out out{verdicts.data(), o[0], o[1]};
+      check_configs(robot, links_per_config, self_pairs, q, out);
+      if (hits[0] <= cap[0] && hits[1] <= cap[1]) break;
+      cap[0] = std::max<size_t>(cap[0], hits[0]);
+      cap[1] = std::max<size_t>(cap[1], hits[1]);
+    }
+    for (int k = 0; k < 2; ++k) {
+      kinds[k]->first.resize(hits[k]);
+      kinds[k]->second.resize(hits[k]);
+      kinds[k]->contacts.resize(hits[k]);
+    }
+    return verdicts;
+  }
+  /// one byte per configuration: 1 iff it collides with the environment or with itself (no pair records come back)
+  std::vector<uint8_t> configuration_flags(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                           const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                           const CollisionRequest& request) {
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    std::vector<uint8_t> verdicts(links_per_config ? robot.hs.size() / links_per_config : 0);
+    hfb_configs_out out{verdicts.data(), {nullptr, nullptr, nullptr, 0, nullptr, nullptr},
+                        {nullptr, nullptr, nullptr, 0, nullptr, nullptr}};
+    check_configs(robot, links_per_config, self_pairs, q, out);
+    return verdicts;
+  }
 
  private:
+  void check_configs(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                     const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const hfb_collision_request& q,
+                     const hfb_configs_out& out) {
+    std::vector<uint32_t> tpl;
+    for (const auto& p : self_pairs) {
+      tpl.push_back(p.first);
+      tpl.push_back(p.second);
+    }
+    const size_t n_configs = links_per_config ? robot.hs.size() / links_per_config : 0;
+    C.check(hfb_env_collide_configs(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), links_per_config,
+                                    self_pairs.size(), tpl.data(), 0, n_configs, &q, &out));
+  }
   void prepare(DynamicAABBTreeCollisionManager& robot, const CollisionRequest& request, hfb_collision_request& q) {
     if (request.num_max_contacts == 0 && request.security_margin != -std::numeric_limits<FCL_REAL>::infinity())
       throw std::invalid_argument("Invalid number of max contacts (current value is 0).");

@@ -256,9 +256,11 @@ def _axis_rotations(axis, ang):
     return R
 
 
-def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, seed=0xFC1 + 6, target_pairs=1_000_000):
+def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, seed=0xFC1 + 6, target_pairs=1_000_000,
+                         joint_range=1.2):
     """A planner's collision query: a seeded chain robot of n_links links (capsules, boxes and two small hulls, joint
-    axes alternating z / y) at n_configs configurations (random base in the room, random joint angles) -- set A,
+    axes alternating z / y) at n_configs configurations (random base in the room, random joint angles, the bending
+    joints within +-joint_range rad: at 2.8 the chain folds back onto itself in some configurations) -- set A,
     n_configs * n_links objects, configuration-major -- against a static environment -- set B: small primitives
     (spheres, boxes, capsules, cylinders of 2-8 cm), about 1 % large boxes (tables, shelves: 0.4-1.2 m), a few OBBRSS
     meshes and a Halfspace floor z <= 0.  `room` (side of the square room, 1.7 m high) defaults to the value that gives
@@ -325,7 +327,7 @@ def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, s
     p = base.copy()
     Rs, Ts = np.empty((K, L, 3, 3)), np.empty((K, L, 3))
     for k in range(L):
-        R = R @ _axis_rotations(2 if k % 2 == 0 else 1, rng.uniform(-1.2, 1.2, K) if k else rng.uniform(0, 2 * np.pi, K))
+        R = R @ _axis_rotations(2 if k % 2 == 0 else 1, rng.uniform(-joint_range, joint_range, K) if k else rng.uniform(0, 2 * np.pi, K))
         axis = R[:, :, 2]
         Rs[:, k] = R
         Ts[:, k] = p + 0.5 * link_len * axis
@@ -336,3 +338,10 @@ def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, s
         geom_a[np.arange(K) * L + k] = s
     return dict(register=register, geom_a=geom_a, tf_a=tf_a, geom_b=geom_b, tf_b=tf_b, room=room, link_len=link_len,
                 n_configs=K, n_links=L)
+
+
+def chain_self_pairs(n_links, skip=2):
+    """the self-pair template of a chain: every link pair (i, j) with j >= i + skip (neighbours touch at their joint
+    and are not checked, as an SRDF disables adjacent links) -> (P, 2) uint32; 105 pairs for 16 links"""
+    i, j = np.triu_indices(n_links, k=skip)
+    return np.stack([i, j], axis=1).astype(np.uint32)

@@ -478,6 +478,50 @@ int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_
                            const hfb_env_out* d_out, void* cuda_stream);
 int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env);
 
+/* ---- a planner's validity check: robot configurations against the resident environment AND against themselves ----
+ * Set A holds n_a = n_configs * links_per_config objects, configuration-major: object g * L + i is link i of
+ * configuration g (L = links_per_config >= 1, n_a % L == 0).  The self-pair template is n_self_pairs pairs of link
+ * indices (i, j), 2 uint32 each (HOST memory): an SRDF's enabled pairs, the collision pairs of a Pinocchio
+ * GeometryModel.  A template with an index >= L, a pair (i, i) or the same unordered pair twice is
+ * HFB_ERR_INVALID_ARGUMENT, and nothing is written; an empty template is allowed.  Only configurations
+ * [first_config, first_config + num_configs) are checked; a range past n_configs is HFB_ERR_INVALID_ARGUMENT.
+ *   Self candidates: per configuration g and template pair (i, j), the pair (g*L + i, g*L + j) when both boxes
+ *     overlap (AABB::overlap, closed intervals; objects without a box take no part) -- the set
+ *     DynamicAABBTreeCollisionManager::collide(callback) over configuration g's L objects hands to a callback that keeps
+ *     only the template's pairs (broadphase_collision_manager.h:104-106).  collide() runs with o1 = g*L + i and
+ *     o2 = g*L + j, in the template's order; a pair whose boxes are apart is never tested, whatever security_margin says.
+ *   Environment candidates: those hfb_env_collide finds for the A objects of the range.
+ *   verdicts (may be null): n_configs bytes, verdicts[g] = 1 iff configuration g has a colliding environment pair or
+ *     a colliding self pair (0 outside the range) -- the OR of what CollisionCallBackDefault leaves in
+ *     data.result.isCollision() (default_broadphase_callbacks.cpp:43-60) after the two reference queries of g.
+ *   env: the colliding environment pairs, byte for byte what hfb_env_collide returns (first: index in A, second: index
+ *     in B).  self: the colliding self pairs (both indices in A), byte for byte what hfb_batch_collide_objects returns
+ *     for them over the table A.  Each kind has its own capacity and counts; all pairs are counted, at most capacity
+ *     of each kind stored, in no particular order.  With verdicts set and both capacities 0, no pair records are
+ *     compacted or downloaded.
+ * An env with no objects still checks the self pairs.  Handles, the env's validity and the request are checked as
+ * hfb_env_collide checks them; security_margin == -inf gives no contacts and all verdicts 0.
+ *   hfb_env_collide_configs: HOST buffers, blocking.
+ *   hfb_env_collide_configs_device: A's handles and poses and every output in DEVICE memory, ordered on `cuda_stream`
+ *     (the template stays in host memory); it blocks as hfb_env_collide_device does.
+ *   hfb_broadphase_config_pairs: the self candidates of boxes `aabbs` (n_a x 6), HOST function, no context: configuration
+ *     by configuration in template order, all counted in *n_pairs, at most `capacity` stored. */
+typedef struct hfb_configs_out {
+  uint8_t* verdicts;
+  hfb_scene_contacts env;
+  hfb_scene_contacts self;
+} hfb_configs_out;
+int hfb_env_collide_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_config,
+                            size_t num_configs, const hfb_collision_request* req, const hfb_configs_out* out);
+int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                   const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                   const hfb_collision_request* req, const hfb_configs_out* d_out, void* cuda_stream);
+int hfb_broadphase_config_pairs(size_t n_a, const double* aabbs, size_t links_per_config, size_t n_self_pairs,
+                                const uint32_t* self_pairs, size_t first_config, size_t num_configs, uint32_t* first,
+                                uint32_t* second, size_t capacity, size_t* n_pairs);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
