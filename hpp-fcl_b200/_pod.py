@@ -162,6 +162,11 @@ class ConfigsOut(C.Structure):  # hfb_configs_out: one verdict byte per configur
     _fields_ = [("verdicts", C.c_void_p), ("env", SceneContacts), ("self", SceneContacts)]
 
 
+class EnvDistanceOut(C.Structure):  # hfb_env_distance_out: per A object the nearest B object, its distance and record
+    _fields_ = [("nearest", C.c_void_p), ("min_distance", C.c_void_p), ("results", C.c_void_p),
+                ("n_candidates", C.c_void_p), ("n_unsupported", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -660,7 +660,7 @@ class DynamicAABBTreeCollisionManager:
 class ResidentEnvironment:
     """A manager's objects kept on the device as set B of the two-set collide (hfb_env): its table, its boxes as of
     construction / update(objs) and the grid over them stay there between queries, as the reference's tree does between
-    setup() and update().  collide() and collide_flags() upload only the robot manager's poses.  close() (or leaving a
+    setup() and update().  collide(), collide_flags(), distance() and clearance() upload only the robot manager's poses.  close() (or leaving a
     `with` block) frees it."""
 
     def __init__(self, manager):
@@ -721,6 +721,28 @@ class ResidentEnvironment:
         back)"""
         h, t, req = self._robot(robot_manager, request)
         return self.engine.env_collide_configs(self._env, h, t, links_per_config, self_pairs, req, 0, 0)[0]
+
+    def distance(self, robot_manager, request=None, max_distance=np.inf):
+        """each robot object's nearest environment object -> (nearest: index in the environment, -1 when none is
+        eligible; min_distance: DBL_MAX when none; the distance records).  distance() runs with a fresh DistanceResult on
+        each pair; the eligible pairs are those at min_distance <= max_distance (>= 0 or inf) and not unsupported; the
+        smallest distance wins, the lowest environment index on ties (include/hppfcl_b200.h, hfb_env_distance)"""
+        h, t, req = self._distance_args(robot_manager, request, max_distance)
+        return self.engine.env_distance(self._env, h, t, req, max_distance)[:3]
+
+    def clearance(self, robot_manager, max_distance=np.inf, request=None):
+        """-> min_distance of distance() alone: each robot object's distance to its nearest environment object (no
+        records come back)"""
+        h, t, req = self._distance_args(robot_manager, request, max_distance)
+        return self.engine.env_distance(self._env, h, t, req, max_distance, records=False)[1]
+
+    @staticmethod
+    def _distance_args(robot_manager, request, max_distance):
+        if not max_distance >= 0:  # (the C++ mirror throws std::invalid_argument)
+            raise ValueError("max_distance must be >= 0 or inf")
+        if robot_manager._stale:
+            robot_manager._refresh()
+        return robot_manager._handles, robot_manager._tfs, (request or DistanceRequest())._pod
 
     def close(self):
         if getattr(self, "_env", None) is not None and getattr(self.engine, "h", None):

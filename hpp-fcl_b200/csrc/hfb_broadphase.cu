@@ -419,6 +419,178 @@ __global__ void __launch_bounds__(128) k_config_pairs(const double* bb, unsigned
   }
 }
 
+// ---- hfb_env_distance's rounds (BpDistState in hfb_broadphase.h) -------------------------------------------------
+// order-preserving key of a double: keys compare as the values do, -0 and +0 share one key (NaN is never keyed)
+__device__ __forceinline__ unsigned long long dist_key(double d) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(d == 0.0 ? 0.0 : d);
+  return (b >> 63) ? ~b : b | 0x8000000000000000ull;
+}
+// the value of a key; the initial keys ~0 and 0 come back as NaN, which no comparison takes
+__device__ __forceinline__ double key_value(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? k & 0x7fffffffffffffffull : ~k));
+}
+__device__ __forceinline__ double dist_radius(double cell, int round, double maxd) {
+  const double r = ldexp(cell, 3 * round);
+  return r < maxd ? r : maxd;
+}
+// box a widened by r on every side, rounded outward: a B box that does not overlap it is more than r away from a
+__device__ __forceinline__ void dist_inflate(const double* a, double r, double* o) {
+  for (int k = 0; k < 3; ++k) {
+    o[k] = __dsub_rd(a[k], r);
+    o[3 + k] = __dadd_ru(a[3 + k], r);
+  }
+}
+// the widened box overlaps every (non-empty) box of B: it reaches past the smallest maximum and the largest minimum
+__device__ __forceinline__ bool dist_covers(const double* a, double r, const unsigned long long* reach) {
+  double o[6];
+  dist_inflate(a, r, o);
+  for (int k = 0; k < 3; ++k)
+    if (o[k] > key_value(reach[k]) || o[3 + k] < key_value(reach[3 + k])) return false;
+  return true;
+}
+__device__ __forceinline__ bool dist_eligible(double d, uint32_t status, double maxd) {
+  return ((status >> 16) & 0xffu) != HFB_PATH_UNSUPPORTED && d <= maxd;  // (NaN: never)
+}
+
+// a fresh record and no best for every A object; the ones in [a_lo, a_hi) open, against all of B in round 0 when
+// their box cannot bound a distance (no box, or a coordinate that is not finite)
+__global__ void __launch_bounds__(256) k_dist_init(const double* ba, unsigned n_a, unsigned a_lo, unsigned a_hi,
+                                                   BpDistState st) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_a) return;
+  uint8_t s = 0;
+  if (i >= a_lo && i < a_hi) {
+    const double* b = ba + 6 * (size_t)i;
+    bool whole = aabb_empty(b);
+    for (int k = 0; k < 6; ++k) whole = whole || !isfinite(b[k]);
+    s = whole ? 2 : 1;
+  }
+  st.state[i] = s;
+  st.key[i] = ~0ull;
+  st.nearest[i] = -1;
+  hfb_distance_result r;  // DistanceResult's initial values (collision_data.h:1090-1096)
+  r.min_distance = DBL_MAX;
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  for (int k = 0; k < 3; ++k) r.p1[k] = r.p2[k] = r.normal[k] = nan;
+  r.b1 = r.b2 = -1;
+  r.status = r.iterations = 0;
+  st.rec[i] = r;
+}
+// B's reach (reach[k]: smallest maximum, reach[3 + k]: largest minimum along axis k; NaN coordinates left out, as they
+// never fail an overlap test)
+__global__ void __launch_bounds__(256) k_dist_reach(const double* bb, unsigned nb, unsigned long long* reach) {
+  unsigned long long v[6] = {~0ull, ~0ull, ~0ull, 0ull, 0ull, 0ull};
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < nb; i += gridDim.x * blockDim.x) {
+    const double* b = bb + 6 * (size_t)i;
+    if (aabb_empty(b)) continue;
+    for (int k = 0; k < 3; ++k) {
+      if (b[3 + k] == b[3 + k]) v[k] = min(v[k], dist_key(b[3 + k]));
+      if (b[k] == b[k]) v[3 + k] = max(v[3 + k], dist_key(b[k]));
+    }
+  }
+  for (int off = 16; off > 0; off >>= 1)
+    for (int k = 0; k < 6; ++k) {
+      const unsigned long long o = __shfl_xor_sync(0xffffffffu, v[k], off);
+      v[k] = k < 3 ? min(v[k], o) : max(v[k], o);
+    }
+  if ((threadIdx.x & 31u) == 0)
+    for (int k = 0; k < 3; ++k) {
+      atomicMin(reach + k, v[k]);
+      atomicMax(reach + 3 + k, v[3 + k]);
+    }
+}
+__global__ void __launch_bounds__(256) k_dist_boxes(const double* ba, unsigned a_lo, unsigned a_hi, const CrossGrid* cgp,
+                                                    double maxd, int round, BpDistState st, double* bq, unsigned* n_open) {
+  const unsigned i = a_lo + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a_hi) return;
+  const double cell = cgp->cell;
+  const double* a = ba + 6 * (size_t)i;
+  uint8_t s = st.state[i];
+  if (round > 0 && s == 2) s = 0;  // it ran against all of B
+  if (round > 0 && s == 1) {
+    const double r = dist_radius(cell, round - 1, maxd);
+    if (st.key[i] <= dist_key(r) || r >= maxd || dist_covers(a, r, st.reach)) s = 0;
+  }
+  st.state[i] = s;
+  double* o = bq + 6 * (size_t)i;
+  if (s == 0) {
+    for (int k = 0; k < 3; ++k) {
+      o[k] = DBL_MAX;
+      o[3 + k] = -DBL_MAX;
+    }
+    return;
+  }
+  st.prev[i] = st.key[i];
+  st.jround[i] = 0xffffffffu;
+  if (s == 2)
+    for (int k = 0; k < 3; ++k) {
+      o[k] = -INFINITY;
+      o[3 + k] = INFINITY;
+    }
+  else
+    dist_inflate(a, dist_radius(cell, round, maxd), o);
+  atomicAdd(n_open, 1u);
+}
+__global__ void __launch_bounds__(256) k_dist_filter(const uint32_t* pf, const uint32_t* ps, const unsigned* n_raw,
+                                                     unsigned cap, const double* ba, const double* bb, unsigned second_base,
+                                                     const CrossGrid* cgp, double maxd, int round, uint32_t* kf, uint32_t* ks,
+                                                     unsigned* n_kept) {
+  const unsigned n = *n_raw < cap ? *n_raw : cap;
+  const unsigned nend = (n + 31u) & ~31u;  // (warp-uniform trip count for the ballots)
+  const double r = round > 0 ? dist_radius(cgp->cell, round - 1, maxd) : 0.0;
+  for (unsigned t = blockIdx.x * blockDim.x + threadIdx.x; t < nend; t += gridDim.x * blockDim.x) {
+    bool keep = false;
+    unsigned i = 0, j = 0;
+    if (t < n) {
+      i = pf[t];
+      j = ps[t];
+      keep = true;
+      if (round > 0) {  // (an object open in this round was open in the one before)
+        double o[6];
+        dist_inflate(ba + 6 * (size_t)i, r, o);
+        keep = !aabb_overlap(o, bb + 6 * (size_t)(j - second_base));
+      }
+    }
+    append_pair(keep, i, j, kf, ks, cap, n_kept);
+  }
+}
+// three passes over a round's records: the smallest key per A object, the lowest index in B at that key, then the
+// winner against the best of the rounds before (strictly better, or equal with a lower index)
+__global__ void __launch_bounds__(256) k_dist_min(const hfb_distance_result* r, const uint32_t* pf, unsigned n, double maxd,
+                                                  unsigned long long* key, unsigned* n_unsupported) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  bool unsup = false;
+  if (p < n) {
+    const double d = r[p].min_distance;
+    const uint32_t status = r[p].status;
+    unsup = ((status >> 16) & 0xffu) == HFB_PATH_UNSUPPORTED;
+    if (dist_eligible(d, status, maxd)) atomicMin(key + pf[p], dist_key(d));
+  }
+  const unsigned m = __ballot_sync(0xffffffffu, unsup);
+  if (m && (threadIdx.x & 31u) == 0) atomicAdd(n_unsupported, (unsigned)__popc(m));
+}
+__global__ void __launch_bounds__(256) k_dist_argmin(const hfb_distance_result* r, const uint32_t* pf, const uint32_t* ps,
+                                                     unsigned n, unsigned second_base, double maxd, BpDistState st) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const double d = r[p].min_distance;
+  const unsigned i = pf[p];
+  if (dist_eligible(d, r[p].status, maxd) && dist_key(d) == st.key[i]) atomicMin(st.jround + i, ps[p] - second_base);
+}
+__global__ void __launch_bounds__(256) k_dist_take(const hfb_distance_result* r, const uint32_t* pf, const uint32_t* ps,
+                                                   unsigned n, unsigned second_base, double maxd, BpDistState st) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const double d = r[p].min_distance;
+  const unsigned i = pf[p], j = ps[p] - second_base;
+  if (!dist_eligible(d, r[p].status, maxd) || dist_key(d) != st.key[i] || j != st.jround[i]) return;
+  // (one pair per A object gets here; nearest -1 compares as the largest index)
+  if (st.key[i] < st.prev[i] || (uint32_t)st.nearest[i] > j) {
+    st.nearest[i] = (int32_t)j;
+    st.rec[i] = r[p];
+  }
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -644,6 +816,84 @@ int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* 
                                               d_second, (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity),
                                               d_n_pairs);
   *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+size_t bp_dist_state_bytes(size_t n_a) { return 2 * up256(n_a * 8) + 2 * up256(n_a * 4) + up256(n_a) + n_a * 96; }
+
+BpDistState bp_dist_state_carve(void* p, size_t n_a, const unsigned long long* reach) {
+  unsigned char* c = static_cast<unsigned char*>(p);
+  BpDistState st;
+  st.reach = reach;
+  st.key = reinterpret_cast<unsigned long long*>(c); c += up256(n_a * 8);
+  st.prev = reinterpret_cast<unsigned long long*>(c); c += up256(n_a * 8);
+  st.nearest = reinterpret_cast<int32_t*>(c); c += up256(n_a * 4);
+  st.jround = reinterpret_cast<uint32_t*>(c); c += up256(n_a * 4);
+  st.state = c; c += up256(n_a);
+  st.rec = reinterpret_cast<hfb_distance_result*>(c);
+  return st;
+}
+
+int bp_dist_reach_launch(size_t n_b, const double* d_bb, unsigned long long* d_reach, int num_sms, cudaStream_t s,
+                         int* launches) {
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(d_reach, 0xff, 24, s)) != cudaSuccess) return (int)e;
+  if ((e = cudaMemsetAsync(d_reach + 3, 0, 24, s)) != cudaSuccess) return (int)e;
+  if (n_b == 0) return 0;
+  if (num_sms < 1) num_sms = 1;
+  size_t nb = (n_b + 255) / 256;
+  if (nb > (size_t)num_sms * 4u) nb = (size_t)num_sms * 4u;
+  k_dist_reach<<<(unsigned)nb, 256, 0, s>>>(d_bb, (unsigned)n_b, d_reach);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_dist_init_launch(size_t n_a, const double* d_ba, size_t a_lo, size_t a_hi, const BpDistState& st, cudaStream_t s,
+                        int* launches) {
+  if (n_a == 0) return 0;
+  k_dist_init<<<(unsigned)((n_a + 255) / 256), 256, 0, s>>>(d_ba, (unsigned)n_a, (unsigned)a_lo, (unsigned)a_hi, st);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_dist_boxes_launch(const double* d_ba, size_t a_lo, size_t a_hi, const BpCrossGrid& g, double max_distance, int round,
+                         const BpDistState& st, double* d_bq, unsigned* d_n_open, cudaStream_t s, int* launches) {
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(d_n_open, 0, sizeof(unsigned), s)) != cudaSuccess) return (int)e;
+  if (a_lo >= a_hi) return 0;
+  k_dist_boxes<<<(unsigned)((a_hi - a_lo + 255) / 256), 256, 0, s>>>(d_ba, (unsigned)a_lo, (unsigned)a_hi,
+                                                                     static_cast<const CrossGrid*>(g.grid), max_distance, round,
+                                                                     st, d_bq, d_n_open);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_dist_filter_launch(const uint32_t* d_first, const uint32_t* d_second, const unsigned* d_n_raw, size_t capacity,
+                          const double* d_ba, const double* d_bb, uint32_t second_base, const BpCrossGrid& g,
+                          double max_distance, int round, uint32_t* d_kept_first, uint32_t* d_kept_second,
+                          unsigned* d_n_kept, int num_sms, cudaStream_t s, int* launches) {
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(d_n_kept, 0, sizeof(unsigned), s)) != cudaSuccess) return (int)e;
+  if (num_sms < 1) num_sms = 1;
+  const unsigned cap = (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity);
+  size_t nb = (capacity + 255) / 256;  // (grid-stride: the count is only known on the device)
+  if (nb > (size_t)num_sms * 8u) nb = (size_t)num_sms * 8u;
+  k_dist_filter<<<(unsigned)(nb ? nb : 1), 256, 0, s>>>(d_first, d_second, d_n_raw, cap, d_ba, d_bb, second_base,
+                                                        static_cast<const CrossGrid*>(g.grid), max_distance, round,
+                                                        d_kept_first, d_kept_second, d_n_kept);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_dist_reduce_launch(const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second, size_t n,
+                          uint32_t second_base, double max_distance, const BpDistState& st, unsigned* d_n_unsupported,
+                          cudaStream_t s, int* launches) {
+  if (n == 0) return 0;
+  const unsigned nb = (unsigned)((n + 255) / 256);
+  k_dist_min<<<nb, 256, 0, s>>>(d_recs, d_first, (unsigned)n, max_distance, st.key, d_n_unsupported);
+  k_dist_argmin<<<nb, 256, 0, s>>>(d_recs, d_first, d_second, (unsigned)n, second_base, max_distance, st);
+  k_dist_take<<<nb, 256, 0, s>>>(d_recs, d_first, d_second, (unsigned)n, second_base, max_distance, st);
+  *launches += 3;
   return (int)cudaGetLastError();
 }
 

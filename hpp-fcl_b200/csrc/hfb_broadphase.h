@@ -55,6 +55,44 @@ int bp_cross_query_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size
 int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
                            size_t num_configs, uint32_t* d_first, uint32_t* d_second, size_t capacity, unsigned* d_n_pairs,
                            int num_sms, cudaStream_t s, int* launches);
+// ---- hfb_env_distance: each A object's nearest B object, found in rounds of growing radius (DESIGN.md §3) ----------
+// Round k runs distance() on the pairs whose B box overlaps the A box inflated by rho_k = min(cell * 8^k, max_distance)
+// (outward rounding) and did not overlap the round before's; an A object is settled once its best eligible distance is
+// <= rho_k, rho_k == max_distance, or its inflated box overlaps every box of B.  A pair a round skips has a box gap,
+// and so a distance, above rho_k.  Per-A state (n_a each, bp_dist_state_bytes(n_a) bytes of the caller's):
+struct BpDistState {
+  unsigned long long* key;   // order-preserving key of the best eligible distance so far; ~0: none
+  unsigned long long* prev;  // key at the start of the round
+  int32_t* nearest;          // index in B of the best pair; -1: none
+  uint32_t* jround;          // the lowest index in B among this round's pairs at `key`
+  uint8_t* state;            // 0: settled or outside the range, 1: open, 2: open for round 0 against all of B
+  hfb_distance_result* rec;  // the record of `nearest` (a fresh DistanceResult while there is none)
+  const unsigned long long* reach;  // B's reach (bp_dist_reach_launch), kept with the env's grid
+};
+size_t bp_dist_state_bytes(size_t n_a);
+BpDistState bp_dist_state_carve(void* p, size_t n_a, const unsigned long long* reach);
+// B's reach from B's boxes, 6 keys: per axis the smallest box maximum and the largest box minimum (an A box widened
+// past both overlaps every box of B); run again after B's boxes change
+int bp_dist_reach_launch(size_t n_b, const double* d_bb, unsigned long long* d_reach, int num_sms, cudaStream_t s,
+                         int* launches);
+// state of all n_a objects from A's boxes d_ba, [a_lo, a_hi) open (a_lo <= a_hi <= n_a)
+int bp_dist_init_launch(size_t n_a, const double* d_ba, size_t a_lo, size_t a_hi, const BpDistState& st, cudaStream_t s,
+                        int* launches);
+// round `round`'s start: objects settled by the round before, then the query boxes d_bq of the open ones (the empty
+// box for the others); *d_n_open = the number of open ones
+int bp_dist_boxes_launch(const double* d_ba, size_t a_lo, size_t a_hi, const BpCrossGrid& g, double max_distance, int round,
+                         const BpDistState& st, double* d_bq, unsigned* d_n_open, cudaStream_t s, int* launches);
+// the first min(*d_n_raw, capacity) candidates (d_first, d_second = second_base + index in B) less the pairs the round
+// before already ran -> (d_kept_first, d_kept_second), counted in *d_n_kept
+int bp_dist_filter_launch(const uint32_t* d_first, const uint32_t* d_second, const unsigned* d_n_raw, size_t capacity,
+                          const double* d_ba, const double* d_bb, uint32_t second_base, const BpCrossGrid& g,
+                          double max_distance, int round, uint32_t* d_kept_first, uint32_t* d_kept_second,
+                          unsigned* d_n_kept, int num_sms, cudaStream_t s, int* launches);
+// the round's n distance() records into the per-A best (smallest eligible distance, then lowest index in B); the
+// candidates that came back HFB_PATH_UNSUPPORTED are added to *d_n_unsupported
+int bp_dist_reduce_launch(const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second, size_t n,
+                          uint32_t second_base, double max_distance, const BpDistState& st, unsigned* d_n_unsupported,
+                          cudaStream_t s, int* launches);
 // hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
                          const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,

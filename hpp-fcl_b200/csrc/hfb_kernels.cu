@@ -23,6 +23,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
+#include <initializer_list>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -907,6 +908,7 @@ struct hfb_ctx {
   DevBuf sc_bb, sc_pf, sc_ps, sc_cnt, sc_out, sc_f, sc_s, sc_rec;  // hfb_scene_collide
   DevBuf sc_flags;                                                 // hfb_env_collide
   DevBuf sc_tpl;                                                   // hfb_env_collide_configs: the self-pair template
+  DevBuf sc_dist, sc_drec;  // hfb_env_distance: the per-A state (hfb::BpDistState), a round's distance() records
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   uint64_t commits = 0, clears = 0;
@@ -921,10 +923,11 @@ struct hfb_env {
   DevBuf h, tf;  // (head + n_b) handles and poses, B from slot `head` on
   DevBuf bb;     // B's boxes
   DevBuf grid;   // hfb::bp_cross_grid_bytes(n_b)
+  DevBuf reach;  // B's reach (hfb::bp_dist_reach_launch): 6 keys, for hfb_env_distance
   std::vector<uint32_t> handles;  // B's handles, checked again after a commit
   uint64_t commits = 0, clears = 0;  // the context's counters when B was last checked
   ~hfb_env() {
-    for (DevBuf* b : {&h, &tf, &bb, &grid}) b->release();
+    for (DevBuf* b : {&h, &tf, &bb, &grid, &reach}) b->release();
   }
 };
 
@@ -1962,7 +1965,8 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   if (c->pin_fix) cudaFreeHost(c->pin_fix);
   for (cudaEvent_t e : c->pipe_events) cudaEventDestroy(e);
   c->bp_scratch.release();
-  for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec, &c->sc_flags})
+  for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec, &c->sc_flags,
+                    &c->sc_dist, &c->sc_drec})
     b->release();
   for (hfb_env* e : c->envs) delete e;
   c->obj_tf.release();
@@ -2479,6 +2483,32 @@ static int after_device_calls(hfb_ctx* ctx, cudaStream_t s) {
   if (ctx->dev_used && ctx->dev_last_stream != s) CK(cudaStreamWaitEvent(s, ctx->dev_done, 0));
   return HFB_OK;
 }
+// The number of candidate pairs is not known in advance: find(cap, &launches) launches a pair finder that counts every
+// candidate in the counter's first word (d_cnt) and stores at most `cap` in each of `lists` (4 bytes per candidate).
+// find_all runs it and reads the counter's first n_words words into `words`; when the count exceeded the lists, they
+// grow to fit it and it runs once more (the second sweep stores what the first counted).
+template <class Find>
+static int find_all(hfb_ctx* ctx, cudaStream_t s, std::initializer_list<DevBuf*> lists, const unsigned* d_cnt, Find find,
+                    unsigned* words, int n_words) {
+  auto lists_cap = [&]() {
+    size_t c = ~(size_t)0;
+    for (DevBuf* b : lists) c = b->cap / 4 < c ? b->cap / 4 : c;
+    return c;
+  };
+  size_t cap = lists_cap();
+  for (int attempt = 0; attempt < 2; ++attempt) {
+    int nl = 0;
+    if (find(cap, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "broadphase launch failed");
+    ctx->stats.kernel_launches += (uint64_t)nl;
+    CK(cudaMemcpyAsync(words, d_cnt, n_words * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    if (words[0] <= cap) break;
+    cap = (size_t)words[0] + words[0] / 8 + 1024;
+    for (DevBuf* b : lists) CK(b->reserve(cap * 4));
+    cap = lists_cap();
+  }
+  return HFB_OK;
+}
 // The part hfb_scene_collide, hfb_scene_collide_sets and hfb_env_collide share, after the upload of the object table
 // (d_h, d_tf: n objects): the boxes of its first n_boxes objects, the candidates (find_pairs(d_bb, pf, ps, capacity,
 // d_count, &launches) launches a pair finder, all pairs counted in *d_count, at most `capacity` stored) and collide() of
@@ -2495,25 +2525,13 @@ static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32
   if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n_boxes, d_h, d_tf, d_bb, s) != 0)
     return fail(ctx, HFB_ERR_CUDA, "k_scene_aabbs launch failed");
   ctx->stats.kernel_launches++;
-  // the number of candidate pairs is not known in advance: a first sweep counts, a second one (if the buffers were too
-  // small) stores
-  size_t cap = ctx->sc_pf.cap / 4 < ctx->sc_ps.cap / 4 ? ctx->sc_pf.cap / 4 : ctx->sc_ps.cap / 4;
-  unsigned cand = 0, words[2] = {0, 0};
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    int nl = 0;
-    if (find_pairs(d_bb, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p), cap, d_cnt, &nl) != 0)
-      return fail(ctx, HFB_ERR_CUDA, "broadphase launch failed");
-    ctx->stats.kernel_launches += (uint64_t)nl;
-    CK(cudaMemcpyAsync(words, d_cnt, (split_out ? 2 : 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    cand = words[0];
-    if (split_out) *split_out = words[1];
-    if (cand <= cap) break;
-    cap = (size_t)cand + cand / 8 + 1024;
-    CK(ctx->sc_pf.reserve(cap * 4));
-    CK(ctx->sc_ps.reserve(cap * 4));
-    cap = ctx->sc_pf.cap / 4 < ctx->sc_ps.cap / 4 ? ctx->sc_pf.cap / 4 : ctx->sc_ps.cap / 4;
-  }
+  unsigned words[2] = {0, 0};
+  auto find = [&](size_t cap, int* nl) {
+    return find_pairs(d_bb, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p), cap, d_cnt, nl);
+  };
+  if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps}, d_cnt, find, words, split_out ? 2 : 1)) return rc;
+  const unsigned cand = words[0];
+  if (split_out) *split_out = words[1];
   *cand_out = cand;
   if (cand == 0 || minus_inf) return HFB_OK;  // collision.cpp:73-76: no contacts under security_margin == -inf
   CK(ctx->sc_out.reserve((size_t)cand * sizeof(hfb_contact)));
@@ -2773,13 +2791,17 @@ static int env_make_room(hfb_ctx* ctx, hfb_env* e, size_t n_a, cudaStream_t s) {
   e->head = head;
   return HFB_OK;
 }
-// the cross grid over B's boxes (scratch: the context's bp_scratch)
+// the cross grid over B's boxes (scratch: the context's bp_scratch) and B's reach
 static int env_build(hfb_ctx* ctx, hfb_env* e, cudaStream_t s) {
   CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(0, e->n_b)));
+  CK(e->reach.reserve(48));
   int nl = 0;
   if (bp_cross_build_launch(e->n_b, static_cast<const double*>(e->bb.p), bp_cross_grid_carve(e->grid.p, e->n_b),
                             ctx->bp_scratch.p, s, &nl) != 0)
     return fail(ctx, HFB_ERR_CUDA, "cross grid launch failed");
+  if (bp_dist_reach_launch(e->n_b, static_cast<const double*>(e->bb.p), static_cast<unsigned long long*>(e->reach.p),
+                           ctx->num_sms, s, &nl) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "k_dist_reach launch failed");
   ctx->stats.kernel_launches += (uint64_t)nl;
   return HFB_OK;
 }
@@ -2933,6 +2955,105 @@ static int env_configs_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t links,
   }
   if (cand == 0 || minus_inf) return HFB_OK;
   return configs_output(ctx, s, cand, split, (uint32_t)n_a, links, n_a / links, out, dev);
+}
+
+// hfb_env_distance's output and cutoff (max_distance >= 0 or +inf), checked before the context is looked at
+static bool env_distance_ok(const hfb_env_distance_out* o, double max_distance) {
+  return o && (o->nearest || o->min_distance || o->results) && max_distance >= 0;
+}
+
+// one distance query of A (already in the table in front of B) against the env: A's boxes, then rounds of candidates
+// within a growing radius (hfb::BpDistState): each round's new pairs through distance() over the table [A; B] and
+// into the per-A best.  Blocks for the candidate counts once per round (per chunk of A, and once more when the lists
+// grow).  Then the outputs (host or device).
+static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a,
+                              const hfb_distance_request* req, double maxd, const hfb_env_distance_out* out, cudaStream_t s,
+                              bool dev) {
+  const size_t n_b = e->n_b, a_lo = first_a < n_a ? first_a : n_a, a_hi = a_lo + (num_a < n_a - a_lo ? num_a : n_a - a_lo);
+  const size_t off = e->head - n_a;
+  const uint32_t* d_h = static_cast<const uint32_t*>(e->h.p) + off;
+  const hfb_transform* d_tf = static_cast<const hfb_transform*>(e->tf.p) + off;
+  const double* bb_b = static_cast<const double*>(e->bb.p);
+  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+  CK(ctx->sc_bb.reserve(n_a * 96));  // A's boxes, then the round's query boxes
+  CK(ctx->sc_cnt.reserve(16));       // candidates, kept candidates, open A objects, unsupported pairs
+  CK(ctx->sc_dist.reserve(bp_dist_state_bytes(n_a)));
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  double* d_ba = static_cast<double*>(ctx->sc_bb.p);
+  double* d_bq = d_ba + 6 * n_a;
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+  const BpDistState st = bp_dist_state_carve(ctx->sc_dist.p, n_a, static_cast<const unsigned long long*>(e->reach.p));
+  int nl = 0;
+  CK(cudaMemsetAsync(d_cnt + 3, 0, sizeof(unsigned), s));
+  if (bp_scene_aabbs_launch(ctx->dview.local_aabbs, ctx->dview.nshapes, n_a, d_h, d_tf, d_ba, s) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "k_scene_aabbs launch failed");
+  ++nl;
+  if (bp_dist_init_launch(n_a, d_ba, a_lo, a_hi, st, s, &nl) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "k_dist_init launch failed");
+  uint64_t total = 0;
+  // a query counts its candidates in 32 bits: the range goes through the grid in chunks of A objects whose pairs with
+  // all of B number fewer than 2^32, so that no round's count can wrap whatever its radius
+  const size_t chunk = n_b ? (0xffffffffull / n_b > 0 ? 0xffffffffull / n_b : 1) : 1;
+  for (int round = 0; n_b && a_lo < a_hi; ++round) {
+    if (bp_dist_boxes_launch(d_ba, a_lo, a_hi, g, maxd, round, st, d_bq, d_cnt + 2, s, &nl) != 0)
+      return fail(ctx, HFB_ERR_CUDA, "k_dist_boxes launch failed");
+    bool open = true;
+    for (size_t c0 = a_lo; open && c0 < a_hi; c0 += chunk) {
+      const size_t c1 = a_hi - c0 > chunk ? c0 + chunk : a_hi;
+      // the chunk's candidates less the pairs the round before ran; the open count is the whole round's
+      unsigned words[3] = {0, 0, 0};
+      auto find = [&](size_t cap, int* launches) {
+        uint32_t* pf = static_cast<uint32_t*>(ctx->sc_pf.p);
+        uint32_t* ps = static_cast<uint32_t*>(ctx->sc_ps.p);
+        int rc = bp_cross_query_reset(g, d_cnt, s);
+        if (!rc)
+          rc = bp_cross_query_launch(n_a, d_bq, c0, c1, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt, ctx->bp_scratch.p,
+                                     ctx->num_sms, s, launches);
+        if (!rc)
+          rc = bp_dist_filter_launch(pf, ps, d_cnt, cap, d_ba, bb_b, (uint32_t)n_a, g, maxd, round,
+                                     static_cast<uint32_t*>(ctx->sc_f.p), static_cast<uint32_t*>(ctx->sc_s.p), d_cnt + 1,
+                                     ctx->num_sms, s, launches);
+        return rc;
+      };
+      if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps, &ctx->sc_f, &ctx->sc_s}, d_cnt, find, words, 3)) return rc;
+      open = words[2] != 0;  // (0: every object of the range is settled)
+      const unsigned kept = words[1];
+      total += kept;
+      if (!open || kept == 0) continue;
+      CK(ctx->sc_drec.reserve((size_t)kept * sizeof(hfb_distance_result)));
+      hfb_object_pairs sc;
+      sc.n_objects = n_a + n_b;
+      sc.object_handles = d_h;
+      sc.object_tfs = d_tf;
+      sc.n_pairs = kept;
+      sc.first = static_cast<const uint32_t*>(ctx->sc_f.p);
+      sc.second = static_cast<const uint32_t*>(ctx->sc_s.p);
+      if (int rc = objects_device<0>(ctx, &sc, req, solver_from_distance_request(*req), CollideP{0, 0},
+                                     bvh_req_of_distance(req), ctx->sc_drec.p, nullptr, s))
+        return rc;
+      if (bp_dist_reduce_launch(static_cast<const hfb_distance_result*>(ctx->sc_drec.p), sc.first, sc.second, kept,
+                                (uint32_t)n_a, maxd, st, d_cnt + 3, s, &nl) != 0)
+        return fail(ctx, HFB_ERR_CUDA, "k_dist_min launch failed");
+    }
+    if (!open) break;
+  }
+  ctx->stats.kernel_launches += (uint64_t)nl;
+  const unsigned n_cand = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
+  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (out->nearest) CK(cudaMemcpyAsync(out->nearest, st.nearest, n_a * 4, kind, s));
+  if (out->min_distance)  // (the records' first field)
+    CK(cudaMemcpy2DAsync(out->min_distance, sizeof(double), st.rec, sizeof(hfb_distance_result), sizeof(double), n_a, kind, s));
+  if (out->results) CK(cudaMemcpyAsync(out->results, st.rec, n_a * sizeof(hfb_distance_result), kind, s));
+  if (out->n_unsupported) CK(cudaMemcpyAsync(out->n_unsupported, d_cnt + 3, sizeof(unsigned), kind, s));
+  if (dev) {
+    if (out->n_candidates)  // (pageable source: staged before the call returns)
+      CK(cudaMemcpyAsync(out->n_candidates, &n_cand, sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    CK(cudaGetLastError());
+    return HFB_OK;
+  }
+  CK(cudaStreamSynchronize(s));
+  if (out->n_candidates) *out->n_candidates = n_cand;
+  return HFB_OK;
 }
 
 extern "C" {
@@ -3138,6 +3259,62 @@ int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
     if (int rc = env_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req, minus_inf,
                                    d_out, s, true))
       return rc;
+  }
+  // the next call that shares the scratch or this table waits for what is still running here
+  CK(cudaEventRecord(ctx->dev_done, s));
+  ctx->dev_used = true;
+  ctx->dev_last_stream = s;
+  return HFB_OK;
+}
+
+// Each A object's nearest B object (hfb_env_distance_out in include/hppfcl_b200.h): the result of
+// NaiveCollisionManager::distance(obj, callback) over B (broadphase_bruteforce.cpp:99-110) with a callback that runs
+// distance() with a fresh DistanceResult on every pair and keeps the smallest eligible one, the first in B's order on
+// ties.  Boxes only skip pairs that cannot be eligible or cannot beat the best found.
+int hfb_env_distance(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                     size_t first_a, size_t num_a, const hfb_distance_request* req, double max_distance,
+                     const hfb_env_distance_out* out) {
+  if (!ctx || !env || !req || !env_distance_ok(out, max_distance) || (n_a && (!handles_a || !tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
+  if (out->n_candidates) *out->n_candidates = 0;
+  if (out->n_unsupported) *out->n_unsupported = 0;
+  if (n_a == 0) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+  const size_t off = env->head - n_a;
+  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  return env_distance_query(ctx, env, n_a, first_a, num_a, req, max_distance, out, s, false);
+}
+
+int hfb_env_distance_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a, const hfb_transform* d_tfs_a,
+                            size_t first_a, size_t num_a, const hfb_distance_request* req, double max_distance,
+                            const hfb_env_distance_out* d_out, void* stream) {
+  if (!ctx || !env || !req || !env_distance_ok(d_out, max_distance) || (n_a && (!d_handles_a || !d_tfs_a)))
+    return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (d_out->n_candidates) CK(cudaMemsetAsync(d_out->n_candidates, 0, sizeof(uint32_t), s));
+  if (d_out->n_unsupported) CK(cudaMemsetAsync(d_out->n_unsupported, 0, sizeof(uint32_t), s));
+  if (n_a) {
+    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+    const size_t off = env->head - n_a;
+    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
+                       cudaMemcpyDeviceToDevice, s));
+    if (int rc = env_distance_query(ctx, env, n_a, first_a, num_a, req, max_distance, d_out, s, true)) return rc;
   }
   // the next call that shares the scratch or this table waits for what is still running here
   CK(cudaEventRecord(ctx->dev_done, s));

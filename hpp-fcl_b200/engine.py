@@ -73,6 +73,8 @@ def load_library(path=None):
     L.hfb_env_destroy.argtypes = [vp, vp]
     L.hfb_env_collide_configs.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, vp]
     L.hfb_env_collide_configs_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, vp, vp]
+    L.hfb_env_distance.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, C.c_double, vp]
+    L.hfb_env_distance_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, C.c_double, vp, vp]
     L.hfb_broadphase_config_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, vp, vp, sz, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
@@ -520,6 +522,34 @@ class Engine:
                                                           tpl.shape[0], _ptr(tpl), first_config,
                                                           n_configs - first_config if num_configs is None else num_configs,
                                                           C.byref(req), C.byref(out), _ptr(stream)))
+
+    def env_distance(self, env, handles_a, tfs_a, req=None, max_distance=np.inf, first_a=0, num_a=None, records=True):
+        """each A object's nearest B object (hfb_env_distance) -> (nearest: index in B or -1, min_distance, records or
+        None with records=False, n_candidates, n_unsupported)"""
+        req = req or P.DistanceRequestPOD()
+        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
+        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
+        if ha.shape[0] != ta.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        na = ha.shape[0]
+        nearest = np.empty(na, dtype=np.int32)
+        dist = np.empty(na, dtype=np.float64)
+        rec = np.empty(na, dtype=P.distance_result_dtype) if records else None
+        nc = np.zeros(2, dtype=np.uint32)
+        out = P.EnvDistanceOut(nearest.ctypes.data, dist.ctypes.data, None if rec is None else rec.ctypes.data,
+                               nc[0:1].ctypes.data, nc[1:2].ctypes.data)
+        self._check(self.L.hfb_env_distance(self.h, env, na, _ptr(ha), _ptr(ta), first_a, na if num_a is None else num_a,
+                                            C.byref(req), float(max_distance), C.byref(out)))
+        return nearest, dist, rec, int(nc[0]), int(nc[1])
+
+    def env_distance_device(self, env, n_a, d_handles_a, d_tfs_a, d_nearest, d_min_distance, d_results, d_n_candidates=None,
+                            d_n_unsupported=None, req=None, max_distance=np.inf, stream=0, first_a=0, num_a=None):
+        """hfb_env_distance_device: A's handles and poses and every output are device pointers, ordered on `stream`"""
+        req = req or P.DistanceRequestPOD()
+        out = P.EnvDistanceOut(d_nearest, d_min_distance, d_results, d_n_candidates, d_n_unsupported)
+        self._check(self.L.hfb_env_distance_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a), first_a,
+                                                   n_a if num_a is None else num_a, C.byref(req), float(max_distance),
+                                                   C.byref(out), _ptr(stream)))
 
     # -- object-table queries: the batched form of the CollisionObject overloads (collision.h:58-61) -----
     @staticmethod

@@ -910,7 +910,8 @@ inline std::vector<hfb_contact> collide(DynamicAABBTreeCollisionManager& manager
 
 /// A manager's objects kept on the device as set B of the two-set collide (hfb_env): the table, the boxes as of
 /// construction / update(objs) and the grid over them stay there between queries, as the reference's tree does between
-/// setup() and update().  collide() and collide_flags() upload only the robot manager's poses.  Owns the hfb_env.
+/// setup() and update().  collide(), collide_flags(), distance() and clearance() upload only the robot manager's poses.
+/// Owns the hfb_env.
 class ResidentEnvironment {
  public:
   explicit ResidentEnvironment(DynamicAABBTreeCollisionManager& manager) : C(manager.C) {
@@ -1015,8 +1016,42 @@ class ResidentEnvironment {
     check_configs(robot, links_per_config, self_pairs, q, out);
     return verdicts;
   }
+  /// each robot object's nearest environment object: nearest[i] (index in the environment, -1 when no pair is
+  /// eligible), min_distance[i] (DBL_MAX when none) and the distance record.  distance() runs with a fresh
+  /// DistanceResult on each pair; the eligible pairs are those at min_distance <= max_distance and not unsupported; the
+  /// smallest distance wins, the lowest environment index on ties (hfb_env_distance).  A max_distance that is NaN or
+  /// negative throws std::invalid_argument.
+  std::vector<hfb_distance_result> distance(DynamicAABBTreeCollisionManager& robot, const DistanceRequest& request,
+                                            std::vector<int32_t>& nearest, std::vector<FCL_REAL>& min_distance,
+                                            FCL_REAL max_distance = std::numeric_limits<FCL_REAL>::infinity()) {
+    std::vector<hfb_distance_result> rec(robot_size(robot, max_distance));
+    nearest.resize(rec.size());
+    min_distance.resize(rec.size());
+    query_distance(robot, request, max_distance, {nearest.data(), min_distance.data(), rec.data(), nullptr, nullptr});
+    return rec;
+  }
+  /// the distances alone: each robot object's distance to its nearest environment object (no records come back)
+  std::vector<FCL_REAL> clearance(DynamicAABBTreeCollisionManager& robot,
+                                  FCL_REAL max_distance = std::numeric_limits<FCL_REAL>::infinity(),
+                                  const DistanceRequest& request = DistanceRequest()) {
+    std::vector<FCL_REAL> d(robot_size(robot, max_distance));
+    query_distance(robot, request, max_distance, {nullptr, d.data(), nullptr, nullptr, nullptr});
+    return d;
+  }
 
  private:
+  size_t robot_size(DynamicAABBTreeCollisionManager& robot, FCL_REAL max_distance) {
+    if (!(max_distance >= 0)) throw std::invalid_argument("max_distance must be >= 0 or inf");
+    if (robot.stale) robot.refresh();
+    return robot.hs.size();
+  }
+  void query_distance(DynamicAABBTreeCollisionManager& robot, const DistanceRequest& request, FCL_REAL max_distance,
+                      const hfb_env_distance_out& out) {
+    hfb_distance_request q;
+    detail::fill(request, q);
+    C.check(hfb_env_distance(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), 0, robot.hs.size(), &q,
+                             max_distance, &out));
+  }
   void check_configs(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
                      const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const hfb_collision_request& q,
                      const hfb_configs_out& out) {

@@ -478,6 +478,52 @@ int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_
                            const hfb_env_out* d_out, void* cuda_stream);
 int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env);
 
+/* ---- each robot object's nearest environment object: distance queries against the resident environment ----------
+ * For every A object i in [first_a, first_a + num_a) (clamped to n_a, as in hfb_env_collide) and every B object j, let
+ * r_ij be distance(o1 = A_i, o2 = B_j) with a fresh DistanceResult: byte for byte the record hfb_batch_distance_objects
+ * writes for the pair (i, n_a + j) over the table [A; B].  A pair is ELIGIBLE when r_ij.min_distance <= max_distance
+ * (a NaN distance never is: DistanceResult::update compares with '>', collision_data.h:1099-1108) and its status does
+ * not carry HFB_PATH_UNSUPPORTED (e.g. a plain BVHModel<OBB>, a plane against a mesh).
+ *   nearest[i]:      the eligible j with the smallest min_distance, compared as doubles (-0.0 == +0.0); the lowest j on
+ *                    a tie; -1 when no pair is eligible.
+ *   min_distance[i]: r_ij.min_distance of that pair; DBL_MAX (DistanceResult's initial value) when there is none.
+ *   results[i]:      the full record r_ij of that pair; when there is none a fresh record: min_distance DBL_MAX, NaN
+ *                    points and normal, b1 = b2 = -1, status and iterations 0.
+ *   Outside the range: -1, DBL_MAX and the fresh record.
+ * This is what NaiveCollisionManager::distance(obj, callback) over B (broadphase_bruteforce.cpp:99-110) computes with
+ * a callback that runs distance() with a fresh result on every pair and keeps the smallest, the first in B's order on
+ * ties.  It is not DistanceCallBackDefault's result: that callback lets each shape pair overwrite min_distance and stops
+ * at the first pair at distance <= 0, so it depends on the manager's visiting order.
+ * max_distance must be >= 0 or +inf (+inf: the nearest object at any range); NaN or a negative value is
+ * HFB_ERR_INVALID_ARGUMENT.  Boxes only skip pairs whose box gap, rounded outward, exceeds max_distance or the best
+ * distance found, relying on a box enclosing its shape as the collide candidates do; B objects without a box take no
+ * part.  The outputs are n_a long; each may be null but not all three.  n_candidates (may be null): the pairs whose
+ * distance() was run, all rounds; n_unsupported (may be null): those of them that came back HFB_PATH_UNSUPPORTED.
+ * Handles, the env's validity and the range are checked as hfb_env_collide checks them, the request as
+ * hfb_batch_distance checks it; a malformed argument writes nothing.
+ *   hfb_env_distance: HOST buffers, blocking.
+ *   hfb_env_distance_device: A's handles and poses and every output in DEVICE memory, ordered on `cuda_stream`.  The
+ *     candidates are found in rounds of growing radius, and the call blocks on `cuda_stream` for each round's candidate
+ *     counts: once per round, and once per round more for every further chunk of the range when n_a' * n_b >= 2^32
+ *     (n_a': the range's length; chunks of floor((2^32 - 1) / n_b) A objects keep the 32-bit counts from wrapping).  A
+ *     round whose candidates outgrow the context's candidate lists counts, grows them and blocks a second time to
+ *     store them.  Growing a context or env buffer (the candidate lists, the round's records, the per-object state,
+ *     the env's table when A has more objects than any query before) allocates device memory, which waits for the
+ *     whole device.  The host form blocks at the same points and at the end. */
+typedef struct hfb_env_distance_out {
+  int32_t* nearest;
+  double* min_distance;
+  hfb_distance_result* results;
+  uint32_t* n_candidates;
+  uint32_t* n_unsupported;
+} hfb_env_distance_out;
+int hfb_env_distance(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                     size_t first_a, size_t num_a, const hfb_distance_request* req, double max_distance,
+                     const hfb_env_distance_out* out);
+int hfb_env_distance_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                            const hfb_transform* d_tfs_a, size_t first_a, size_t num_a, const hfb_distance_request* req,
+                            double max_distance, const hfb_env_distance_out* d_out, void* cuda_stream);
+
 /* ---- a planner's validity check: robot configurations against the resident environment AND against themselves ----
  * Set A holds n_a = n_configs * links_per_config objects, configuration-major: object g * L + i is link i of
  * configuration g (L = links_per_config >= 1, n_a % L == 0).  The self-pair template is n_self_pairs pairs of link
