@@ -167,6 +167,12 @@ class EnvDistanceOut(C.Structure):  # hfb_env_distance_out: per A object the nea
                 ("n_candidates", C.c_void_p), ("n_unsupported", C.c_void_p)]
 
 
+class ConfigsDistanceOut(C.Structure):  # hfb_configs_distance_out: per configuration its nearest pair, environment or self
+    _fields_ = [("kind", C.c_void_p), ("first", C.c_void_p), ("second", C.c_void_p), ("min_distance", C.c_void_p),
+                ("results", C.c_void_p), ("n_env_candidates", C.c_void_p), ("n_self_candidates", C.c_void_p),
+                ("n_unsupported", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -660,8 +660,8 @@ class DynamicAABBTreeCollisionManager:
 class ResidentEnvironment:
     """A manager's objects kept on the device as set B of the two-set collide (hfb_env): its table, its boxes as of
     construction / update(objs) and the grid over them stay there between queries, as the reference's tree does between
-    setup() and update().  collide(), collide_flags(), distance() and clearance() upload only the robot manager's poses.  close() (or leaving a
-    `with` block) frees it."""
+    setup() and update().  Its queries (collide(), distance() and their forms per configuration) upload only the robot
+    manager's poses.  close() (or leaving a `with` block) frees it."""
 
     def __init__(self, manager):
         if manager._stale:
@@ -735,6 +735,37 @@ class ResidentEnvironment:
         records come back)"""
         h, t, req = self._distance_args(robot_manager, request, max_distance)
         return self.engine.env_distance(self._env, h, t, req, max_distance, records=False)[1]
+
+    def distance_configurations(self, robot_manager, links_per_config, self_pairs, request=None, max_distance=np.inf):
+        """A planner's clearance: the robot manager holds configurations of links_per_config objects each,
+        configuration-major, and self_pairs is the template of link pairs (i, j) each configuration checks against
+        itself.  -> per configuration its nearest pair over the environment pairs and the template's self pairs: (kind:
+        0 environment, 1 self, -1 none eligible; first: index in the robot manager; second: index in the environment
+        for kind 0, in the robot manager for kind 1; min_distance: DBL_MAX when none; the distance records).  The
+        eligible pairs and the argmin are those of distance(); on a tie an environment pair beats a self pair, and
+        earlier links and template entries beat later ones (include/hppfcl_b200.h, hfb_env_distance_configs)"""
+        h, t, req = self._distance_args(robot_manager, request, max_distance)
+        tpl = self._template_args(links_per_config, self_pairs)
+        return self.engine.env_distance_configs(self._env, h, t, links_per_config, tpl, req, max_distance)[:5]
+
+    def configuration_clearance(self, robot_manager, links_per_config, self_pairs, max_distance=np.inf, request=None):
+        """-> min_distance of distance_configurations() alone: each configuration's clearance (no records come back)"""
+        h, t, req = self._distance_args(robot_manager, request, max_distance)
+        tpl = self._template_args(links_per_config, self_pairs)
+        return self.engine.env_distance_configs(self._env, h, t, links_per_config, tpl, req, max_distance,
+                                                records=False)[3]
+
+    @staticmethod
+    def _template_args(links_per_config, self_pairs):
+        """the template as the C ABI takes it; one the C ABI refuses raises ValueError (the C++ mirror throws
+        std::invalid_argument)"""
+        tpl = np.asarray(self_pairs, dtype=np.int64).reshape(-1, 2)
+        lpc = int(links_per_config)
+        key = np.sort(tpl, axis=1)
+        if ((tpl < 0) | (tpl >= lpc)).any() or (tpl[:, 0] == tpl[:, 1]).any() or len(np.unique(key, axis=0)) != len(key):
+            raise ValueError("self-pair template: a link index out of range, a link paired with itself or a pair listed "
+                             "twice")
+        return tpl.astype(np.uint32)
 
     @staticmethod
     def _distance_args(robot_manager, request, max_distance):

@@ -591,6 +591,114 @@ __global__ void __launch_bounds__(256) k_dist_take(const hfb_distance_result* r,
   }
 }
 
+// ---- hfb_env_distance_configs (BpConfigDist in hfb_broadphase.h) --------------------------------------------------
+// the self pairs config_dist_pair runs, one thread per (configuration, template entry), each with its template entry in
+// `entry` at its position in the list (the reduction's tie order)
+__global__ void __launch_bounds__(128) k_config_dist_pairs(const double* bb, unsigned links, const uint32_t* tpl,
+                                                           unsigned n_tpl, unsigned g0, size_t total, double maxd,
+                                                           uint32_t* first, uint32_t* second, uint32_t* entry,
+                                                           unsigned capacity, unsigned* n_pairs) {
+  const size_t tend = (total + 31u) & ~(size_t)31;  // (warp-uniform trip count for the ballots)
+  const unsigned lane = threadIdx.x & 31u;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < tend; t += (size_t)gridDim.x * blockDim.x) {
+    bool hit = false;
+    uint32_t a = 0, b = 0;
+    if (t < total) hit = config_dist_pair(bb, links, tpl, n_tpl, g0, t, maxd, &a, &b);
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if (!m) continue;
+    unsigned base = 0;
+    if (lane == (unsigned)(__ffs(m) - 1)) base = atomicAdd(n_pairs, (unsigned)__popc(m));
+    base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
+    const unsigned pos = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+    if (hit && pos < capacity) {
+      first[pos] = a;
+      second[pos] = b;
+      entry[pos] = (uint32_t)(t % n_tpl);
+    }
+  }
+}
+__global__ void __launch_bounds__(256) k_cfg_init(unsigned n, BpConfigDist cs) {
+  const unsigned g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  cs.key[g] = ~0ull;
+  cs.ord[g] = ~0ull;
+  cs.kind[g] = -1;
+  cs.first[g] = cs.second[g] = 0xffffffffu;
+  hfb_distance_result r;  // DistanceResult's initial values, as k_dist_init writes them
+  r.min_distance = DBL_MAX;
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  for (int k = 0; k < 3; ++k) r.p1[k] = r.p2[k] = r.normal[k] = nan;
+  r.b1 = r.b2 = -1;
+  r.status = r.iterations = 0;
+  cs.rec[g] = r;
+}
+// the items of one chunk's reduction: t < n_links is link a_lo + t with the best its rounds left (ordinal: the link
+// index within its configuration), the rest are self records (ordinal L + template entry); false when not eligible
+struct CfgItems {
+  unsigned a_lo, n_links, links, n_self;
+  const hfb_distance_result* r;
+  const uint32_t *pf, *ps, *pk;
+  double maxd;
+};
+__device__ __forceinline__ bool cfg_item(const BpDistState& st, const CfgItems& it, size_t t, unsigned* g,
+                                         unsigned long long* key, unsigned long long* ord) {
+  if (t < it.n_links) {
+    const unsigned i = it.a_lo + (unsigned)t;
+    *g = i / it.links;
+    *ord = i - *g * it.links;
+    *key = st.key[i];
+    return *key != ~0ull;
+  }
+  const unsigned p = (unsigned)(t - it.n_links);
+  *g = it.pf[p] / it.links;
+  *ord = (unsigned long long)it.links + it.pk[p];
+  const double d = it.r[p].min_distance;
+  *key = dist_key(d);
+  return dist_eligible(d, it.r[p].status, it.maxd);
+}
+// three passes as k_dist_min / k_dist_argmin / k_dist_take: the smallest key per configuration, the lowest ordinal at
+// that key, then the gather of the winner
+__global__ void __launch_bounds__(256) k_cfg_min(BpDistState st, CfgItems it, BpConfigDist cs, unsigned* n_unsupported) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  bool unsup = false;
+  if (t < (size_t)it.n_links + it.n_self) {
+    unsigned g;
+    unsigned long long key, ord;
+    if (cfg_item(st, it, t, &g, &key, &ord)) atomicMin(cs.key + g, key);
+    unsup = t >= it.n_links && ((it.r[t - it.n_links].status >> 16) & 0xffu) == HFB_PATH_UNSUPPORTED;
+  }
+  const unsigned m = __ballot_sync(0xffffffffu, unsup);
+  if (m && (threadIdx.x & 31u) == 0) atomicAdd(n_unsupported, (unsigned)__popc(m));
+}
+__global__ void __launch_bounds__(256) k_cfg_argmin(BpDistState st, CfgItems it, BpConfigDist cs) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (size_t)it.n_links + it.n_self) return;
+  unsigned g;
+  unsigned long long key, ord;
+  if (cfg_item(st, it, t, &g, &key, &ord) && key == cs.key[g]) atomicMin(cs.ord + g, ord);
+}
+__global__ void __launch_bounds__(256) k_cfg_take(BpDistState st, CfgItems it, BpConfigDist cs) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (size_t)it.n_links + it.n_self) return;
+  unsigned g;
+  unsigned long long key, ord;
+  if (!cfg_item(st, it, t, &g, &key, &ord) || key != cs.key[g] || ord != cs.ord[g]) return;
+  // (ordinals are unique within a configuration: one item per configuration gets here)
+  if (t < it.n_links) {
+    const unsigned i = it.a_lo + (unsigned)t;
+    cs.kind[g] = 0;
+    cs.first[g] = i;
+    cs.second[g] = (uint32_t)st.nearest[i];
+    cs.rec[g] = st.rec[i];
+  } else {
+    const unsigned p = (unsigned)(t - it.n_links);
+    cs.kind[g] = 1;
+    cs.first[g] = it.pf[p];
+    cs.second[g] = it.ps[p];
+    cs.rec[g] = it.r[p];
+  }
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -893,6 +1001,62 @@ int bp_dist_reduce_launch(const hfb_distance_result* d_recs, const uint32_t* d_f
   k_dist_min<<<nb, 256, 0, s>>>(d_recs, d_first, (unsigned)n, max_distance, st.key, d_n_unsupported);
   k_dist_argmin<<<nb, 256, 0, s>>>(d_recs, d_first, d_second, (unsigned)n, second_base, max_distance, st);
   k_dist_take<<<nb, 256, 0, s>>>(d_recs, d_first, d_second, (unsigned)n, second_base, max_distance, st);
+  *launches += 3;
+  return (int)cudaGetLastError();
+}
+
+size_t bp_config_dist_bytes(size_t n_configs) { return 2 * up256(n_configs * 8) + 2 * up256(n_configs * 4) + up256(n_configs) + n_configs * 96; }
+
+BpConfigDist bp_config_dist_carve(void* p, size_t n_configs) {
+  unsigned char* c = static_cast<unsigned char*>(p);
+  BpConfigDist cs;
+  cs.key = reinterpret_cast<unsigned long long*>(c); c += up256(n_configs * 8);
+  cs.ord = reinterpret_cast<unsigned long long*>(c); c += up256(n_configs * 8);
+  cs.first = reinterpret_cast<uint32_t*>(c); c += up256(n_configs * 4);
+  cs.second = reinterpret_cast<uint32_t*>(c); c += up256(n_configs * 4);
+  cs.kind = reinterpret_cast<int8_t*>(c); c += up256(n_configs);
+  cs.rec = reinterpret_cast<hfb_distance_result*>(c);
+  return cs;
+}
+
+int bp_config_dist_init_launch(size_t n_configs, const BpConfigDist& cs, cudaStream_t s, int* launches) {
+  if (n_configs == 0) return 0;
+  k_cfg_init<<<(unsigned)((n_configs + 255) / 256), 256, 0, s>>>((unsigned)n_configs, cs);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_config_dist_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
+                                size_t num_configs, double max_distance, uint32_t* d_first, uint32_t* d_second,
+                                uint32_t* d_entry, size_t capacity, unsigned* d_n_pairs, int num_sms, cudaStream_t s,
+                                int* launches) {
+  cudaError_t e;
+  if ((e = cudaMemsetAsync(d_n_pairs, 0, sizeof(unsigned), s)) != cudaSuccess) return (int)e;
+  const size_t total = num_configs * n_tpl;
+  if (total == 0) return 0;
+  if (num_sms < 1) num_sms = 1;
+  size_t nb = (total + 127) / 128;
+  if (nb > (size_t)num_sms * 16u) nb = (size_t)num_sms * 16u;
+  k_config_dist_pairs<<<(unsigned)nb, 128, 0, s>>>(d_aabbs, (unsigned)links, d_tpl, (unsigned)n_tpl, (unsigned)g0, total,
+                                                   max_distance, d_first, d_second, d_entry,
+                                                   (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity),
+                                                   d_n_pairs);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_config_dist_reduce_launch(const BpDistState& st, size_t a_lo, size_t a_hi, size_t links,
+                                 const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second,
+                                 const uint32_t* d_entry, size_t n_self, double max_distance, const BpConfigDist& cs,
+                                 unsigned* d_n_unsupported, cudaStream_t s, int* launches) {
+  const CfgItems it{(unsigned)a_lo, (unsigned)(a_hi - a_lo), (unsigned)links, (unsigned)n_self, d_recs, d_first, d_second,
+                    d_entry, max_distance};
+  const size_t n = (a_hi - a_lo) + n_self;
+  if (n == 0) return 0;
+  const unsigned nb = (unsigned)((n + 255) / 256);
+  k_cfg_min<<<nb, 256, 0, s>>>(st, it, cs, d_n_unsupported);
+  k_cfg_argmin<<<nb, 256, 0, s>>>(st, it, cs);
+  k_cfg_take<<<nb, 256, 0, s>>>(st, it, cs);
   *launches += 3;
   return (int)cudaGetLastError();
 }

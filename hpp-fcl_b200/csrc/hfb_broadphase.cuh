@@ -465,4 +465,62 @@ inline size_t broadphase_config_pairs_host(const double* bb, uint32_t links, con
   return count;
 }
 
+// ---- self pairs within configurations for distance: the pairs whose distance() must run --------------------------
+// a - r rounded down and a + r rounded up (r >= 0): __dsub_rd / __dadd_ru on the device.  On the host the nearest sum
+// and its exact rounding error (TwoSum, no multiplication, so no contraction can change it) give the same value: one
+// step outward when the error lies outward.  An overflow to +-inf already lies outward (its error is NaN).
+HFB_HD double sub_rd(double a, double r) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rd(a, r);
+#else
+  const double s = a - r, z = s - a, e = (a - (s - z)) - (r + z);
+  return e < 0 ? nextafter(s, -INFINITY) : s;
+#endif
+}
+HFB_HD double add_ru(double a, double r) {
+#ifdef __CUDA_ARCH__
+  return __dadd_ru(a, r);
+#else
+  const double s = a + r, z = s - a, e = (a - (s - z)) + (r - z);
+  return e > 0 ? nextafter(s, INFINITY) : s;
+#endif
+}
+// self pair t as in config_pair; true when its distance() runs: unless both boxes exist and are finite and link j's box
+// does not overlap link i's box widened by max_distance, rounded outward (the test k_dist_filter applies with
+// dist_inflate) -- then the box gap, and so the distance, exceeds max_distance.  At max_distance = inf all run.
+HFB_HD bool config_dist_pair(const double* bb, uint32_t links, const uint32_t* tpl, uint32_t n_pairs, uint32_t g0, size_t t,
+                             double maxd, uint32_t* a, uint32_t* b) {
+  const size_t g = g0 + t / n_pairs, k = t % n_pairs;
+  *a = (uint32_t)(g * links + tpl[2 * k]);
+  *b = (uint32_t)(g * links + tpl[2 * k + 1]);
+  const double* x = bb + 6 * (size_t)*a;
+  const double* y = bb + 6 * (size_t)*b;
+  if (aabb_empty(x) || aabb_empty(y)) return true;
+  for (int c = 0; c < 6; ++c)
+    if (!isfinite(x[c]) || !isfinite(y[c])) return true;
+  double o[6];
+  for (int c = 0; c < 3; ++c) {
+    o[c] = sub_rd(x[c], maxd);
+    o[3 + c] = add_ru(x[3 + c], maxd);
+  }
+  return aabb_overlap(o, y);
+}
+// the pairs config_dist_pair runs for configurations [g0, g0 + num_configs), configuration by configuration in template
+// order; returns their number (all of them are counted, at most `capacity` stored)
+inline size_t broadphase_config_distance_pairs_host(const double* bb, uint32_t links, const uint32_t* tpl, uint32_t n_pairs,
+                                                    uint32_t g0, size_t num_configs, double maxd, uint32_t* first,
+                                                    uint32_t* second, size_t capacity) {
+  size_t count = 0;
+  for (size_t t = 0; t < num_configs * n_pairs; ++t) {
+    uint32_t a, b;
+    if (!config_dist_pair(bb, links, tpl, n_pairs, g0, t, maxd, &a, &b)) continue;
+    if (count < capacity) {
+      first[count] = a;
+      second[count] = b;
+    }
+    ++count;
+  }
+  return count;
+}
+
 }  // namespace hfb

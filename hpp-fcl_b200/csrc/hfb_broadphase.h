@@ -93,6 +93,36 @@ int bp_dist_filter_launch(const uint32_t* d_first, const uint32_t* d_second, con
 int bp_dist_reduce_launch(const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second, size_t n,
                           uint32_t second_base, double max_distance, const BpDistState& st, unsigned* d_n_unsupported,
                           cudaStream_t s, int* launches);
+// ---- hfb_env_distance_configs: each configuration's nearest pair, environment or self (DESIGN.md §3) ---------------
+// After the rounds above over the range's links, the self pairs config_dist_pair runs go through distance(); the best
+// per configuration is then taken over the links' winners (ordinal: link index i) and the self records (ordinal L + k,
+// k the template entry), smallest key first, then lowest ordinal.  Per-configuration state, n_configs each
+// (bp_config_dist_bytes(n_configs) bytes of the caller's):
+struct BpConfigDist {
+  unsigned long long* key;  // order-preserving key of the best eligible distance; ~0: none
+  unsigned long long* ord;  // the lowest ordinal at `key`
+  uint32_t* first;          // the winner's index in A; UINT32_MAX: none
+  uint32_t* second;         // its index in B (kind 0) or in A (kind 1); UINT32_MAX: none
+  int8_t* kind;             // 0: environment pair, 1: self pair, -1: none
+  hfb_distance_result* rec; // the winner's record (a fresh DistanceResult while there is none)
+};
+size_t bp_config_dist_bytes(size_t n_configs);
+BpConfigDist bp_config_dist_carve(void* p, size_t n_configs);
+// every configuration without a winner
+int bp_config_dist_init_launch(size_t n_configs, const BpConfigDist& cs, cudaStream_t s, int* launches);
+// the self pairs of configurations [g0, g0 + num_configs) that config_dist_pair runs -> (d_first, d_second, d_entry: the
+// template entry), at most `capacity` stored, all counted in *d_n_pairs (cleared first)
+int bp_config_dist_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
+                                size_t num_configs, double max_distance, uint32_t* d_first, uint32_t* d_second,
+                                uint32_t* d_entry, size_t capacity, unsigned* d_n_pairs, int num_sms, cudaStream_t s,
+                                int* launches);
+// the winners of the configurations that links [a_lo, a_hi) make up (whole configurations), from the links' state st
+// and the n_self records of their self pairs (d_first, d_second, d_entry as bp_config_dist_pairs_launch stored them);
+// the self records that came back HFB_PATH_UNSUPPORTED are added to *d_n_unsupported
+int bp_config_dist_reduce_launch(const BpDistState& st, size_t a_lo, size_t a_hi, size_t links,
+                                 const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second,
+                                 const uint32_t* d_entry, size_t n_self, double max_distance, const BpConfigDist& cs,
+                                 unsigned* d_n_unsupported, cudaStream_t s, int* launches);
 // hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
                          const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,

@@ -909,6 +909,7 @@ struct hfb_ctx {
   DevBuf sc_flags;                                                 // hfb_env_collide
   DevBuf sc_tpl;                                                   // hfb_env_collide_configs: the self-pair template
   DevBuf sc_dist, sc_drec;  // hfb_env_distance: the per-A state (hfb::BpDistState), a round's distance() records
+  DevBuf sc_cdist;          // hfb_env_distance_configs: the per-configuration state (hfb::BpConfigDist)
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   uint64_t commits = 0, clears = 0;
@@ -1966,7 +1967,7 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   for (cudaEvent_t e : c->pipe_events) cudaEventDestroy(e);
   c->bp_scratch.release();
   for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec, &c->sc_flags,
-                    &c->sc_dist, &c->sc_drec})
+                    &c->sc_dist, &c->sc_drec, &c->sc_cdist})
     b->release();
   for (hfb_env* e : c->envs) delete e;
   c->obj_tf.release();
@@ -2687,6 +2688,24 @@ int hfb_broadphase_config_pairs(size_t n_a, const double* aabbs, size_t links_pe
   return HFB_OK;
 }
 
+// the self pairs whose distance() hfb_env_distance_configs runs (config_dist_pair), for every configuration of the range
+int hfb_broadphase_config_distance_pairs(size_t n_a, const double* aabbs, size_t links_per_config, size_t n_self_pairs,
+                                         const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                         double max_distance, uint32_t* first, uint32_t* second, size_t capacity,
+                                         size_t* n_pairs) {
+  if ((n_a && !aabbs) || !n_pairs || (capacity && (!first || !second)) || (n_self_pairs && !self_pairs) ||
+      n_a > 0xffffffffull || n_self_pairs > 0xffffffffull || !(max_distance >= 0))
+    return HFB_ERR_INVALID_ARGUMENT;
+  const size_t L = links_per_config;
+  if (L == 0 || n_a % L || first_config > n_a / L || num_configs > n_a / L - first_config ||
+      config_template_error(L, n_self_pairs, self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  *n_pairs = broadphase_config_distance_pairs_host(aabbs, (uint32_t)L, self_pairs, (uint32_t)n_self_pairs,
+                                                   (uint32_t)first_config, num_configs, max_distance, first, second,
+                                                   capacity);
+  return HFB_OK;
+}
+
 int hfb_broadphase_cross_pairs_device(hfb_ctx* ctx, size_t n_a, const double* d_aabbs_a, size_t first_a, size_t num_a,
                                       size_t n_b, const double* d_aabbs_b, uint32_t* d_first, uint32_t* d_second,
                                       size_t capacity, uint32_t* d_n_pairs, void* stream) {
@@ -2962,14 +2981,15 @@ static bool env_distance_ok(const hfb_env_distance_out* o, double max_distance) 
   return o && (o->nearest || o->min_distance || o->results) && max_distance >= 0;
 }
 
-// one distance query of A (already in the table in front of B) against the env: A's boxes, then rounds of candidates
-// within a growing radius (hfb::BpDistState): each round's new pairs through distance() over the table [A; B] and
-// into the per-A best.  Blocks for the candidate counts once per round (per chunk of A, and once more when the lists
-// grow).  Then the outputs (host or device).
-static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a,
-                              const hfb_distance_request* req, double maxd, const hfb_env_distance_out* out, cudaStream_t s,
-                              bool dev) {
-  const size_t n_b = e->n_b, a_lo = first_a < n_a ? first_a : n_a, a_hi = a_lo + (num_a < n_a - a_lo ? num_a : n_a - a_lo);
+// the rounds of a distance query of A (already in the table in front of B) against the env for A objects [a_lo, a_hi):
+// A's boxes (ctx->sc_bb), then rounds of candidates within a growing radius (hfb::BpDistState, in ctx->sc_dist): each
+// round's new pairs through distance() over the table [A; B] and into the per-A best.  Blocks for the candidate counts
+// once per round (per chunk of A, and once more when the lists grow).  *st: the per-A state; *n_cand: the pairs whose
+// distance() ran (clamped to 32 bits); the unsupported ones are counted in ctx->sc_cnt's fourth word.
+static int env_distance_rounds(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t a_lo, size_t a_hi,
+                               const hfb_distance_request* req, double maxd, cudaStream_t s, BpDistState* st_out,
+                               unsigned* n_cand) {
+  const size_t n_b = e->n_b;
   const size_t off = e->head - n_a;
   const uint32_t* d_h = static_cast<const uint32_t*>(e->h.p) + off;
   const hfb_transform* d_tf = static_cast<const hfb_transform*>(e->tf.p) + off;
@@ -3038,7 +3058,20 @@ static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first
     if (!open) break;
   }
   ctx->stats.kernel_launches += (uint64_t)nl;
-  const unsigned n_cand = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
+  *st_out = st;
+  *n_cand = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
+  return HFB_OK;
+}
+
+// one distance query of A against the env: the rounds over the range, then the per-A outputs (host or device)
+static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a,
+                              const hfb_distance_request* req, double maxd, const hfb_env_distance_out* out, cudaStream_t s,
+                              bool dev) {
+  const size_t a_lo = first_a < n_a ? first_a : n_a, a_hi = a_lo + (num_a < n_a - a_lo ? num_a : n_a - a_lo);
+  BpDistState st;
+  unsigned n_cand = 0;
+  if (int rc = env_distance_rounds(ctx, e, n_a, a_lo, a_hi, req, maxd, s, &st, &n_cand)) return rc;
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
   const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   if (out->nearest) CK(cudaMemcpyAsync(out->nearest, st.nearest, n_a * 4, kind, s));
   if (out->min_distance)  // (the records' first field)
@@ -3053,6 +3086,90 @@ static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first
   }
   CK(cudaStreamSynchronize(s));
   if (out->n_candidates) *out->n_candidates = n_cand;
+  return HFB_OK;
+}
+
+// hfb_env_distance_configs' output and cutoff, checked before the context is looked at
+static bool configs_distance_ok(const hfb_configs_distance_out* o, double max_distance) {
+  return o && (o->kind || o->min_distance || o->results) && max_distance >= 0;
+}
+
+// one configurations distance query of A (already in the table in front of B, the template in ctx->sc_tpl): the rounds
+// over the range's links, then per chunk of configurations the self pairs config_dist_pair runs, distance() of them
+// over the table [A; B], and the winner of each configuration from its links' winners and its self records (in
+// ctx->sc_cdist).  Blocks for the self candidate count once per chunk (and once more when the lists grow).  Then the
+// outputs (host or device).
+static int env_distance_configs_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t links, size_t n_tpl, size_t g0,
+                                      size_t ng, const hfb_distance_request* req, double maxd,
+                                      const hfb_configs_distance_out* out, cudaStream_t s, bool dev) {
+  const size_t n_b = e->n_b, n_configs = n_a / links;
+  BpDistState st;
+  unsigned n_env = 0;
+  if (int rc = env_distance_rounds(ctx, e, n_a, g0 * links, (g0 + ng) * links, req, maxd, s, &st, &n_env)) return rc;
+  CK(ctx->sc_cdist.reserve(bp_config_dist_bytes(n_configs)));
+  const BpConfigDist cs = bp_config_dist_carve(ctx->sc_cdist.p, n_configs);
+  const size_t off = e->head - n_a;
+  const double* d_ba = static_cast<const double*>(ctx->sc_bb.p);  // (A's boxes, from the rounds)
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+  int nl = 0;
+  if (bp_config_dist_init_launch(n_configs, cs, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_cfg_init launch failed");
+  uint64_t total = 0;
+  // the self candidates are counted in 32 bits: chunks of configurations whose template entries number fewer than 2^32
+  // (whole configurations, so that each chunk's winners are final)
+  const size_t chunk = n_tpl ? 0xffffffffull / n_tpl : (ng ? ng : 1);
+  for (size_t c0 = g0; c0 < g0 + ng; c0 += chunk) {
+    const size_t c1 = g0 + ng - c0 > chunk ? c0 + chunk : g0 + ng;
+    unsigned kept = 0;
+    if (n_tpl) {
+      auto find = [&](size_t cap, int* launches) {
+        return bp_config_dist_pairs_launch(d_ba, links, d_tpl, n_tpl, c0, c1 - c0, maxd, static_cast<uint32_t*>(ctx->sc_pf.p),
+                                           static_cast<uint32_t*>(ctx->sc_ps.p), static_cast<uint32_t*>(ctx->sc_f.p), cap,
+                                           d_cnt, ctx->num_sms, s, launches);
+      };
+      unsigned words[1] = {0};
+      if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps, &ctx->sc_f}, d_cnt, find, words, 1)) return rc;
+      kept = words[0];
+      total += kept;
+    }
+    if (kept) {
+      CK(ctx->sc_drec.reserve((size_t)kept * sizeof(hfb_distance_result)));
+      hfb_object_pairs sc;
+      sc.n_objects = n_a + n_b;
+      sc.object_handles = static_cast<const uint32_t*>(e->h.p) + off;
+      sc.object_tfs = static_cast<const hfb_transform*>(e->tf.p) + off;
+      sc.n_pairs = kept;
+      sc.first = static_cast<const uint32_t*>(ctx->sc_pf.p);
+      sc.second = static_cast<const uint32_t*>(ctx->sc_ps.p);
+      if (int rc = objects_device<0>(ctx, &sc, req, solver_from_distance_request(*req), CollideP{0, 0},
+                                     bvh_req_of_distance(req), ctx->sc_drec.p, nullptr, s))
+        return rc;
+    }
+    if (bp_config_dist_reduce_launch(st, c0 * links, c1 * links, links, static_cast<const hfb_distance_result*>(ctx->sc_drec.p),
+                                     static_cast<const uint32_t*>(ctx->sc_pf.p), static_cast<const uint32_t*>(ctx->sc_ps.p),
+                                     static_cast<const uint32_t*>(ctx->sc_f.p), kept, maxd, cs, d_cnt + 3, s, &nl) != 0)
+      return fail(ctx, HFB_ERR_CUDA, "k_cfg_min launch failed");
+  }
+  ctx->stats.kernel_launches += (uint64_t)nl;
+  const unsigned n_self = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
+  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (out->kind) CK(cudaMemcpyAsync(out->kind, cs.kind, n_configs, kind, s));
+  if (out->first) CK(cudaMemcpyAsync(out->first, cs.first, n_configs * 4, kind, s));
+  if (out->second) CK(cudaMemcpyAsync(out->second, cs.second, n_configs * 4, kind, s));
+  if (out->min_distance)  // (the records' first field)
+    CK(cudaMemcpy2DAsync(out->min_distance, sizeof(double), cs.rec, sizeof(hfb_distance_result), sizeof(double), n_configs,
+                         kind, s));
+  if (out->results) CK(cudaMemcpyAsync(out->results, cs.rec, n_configs * sizeof(hfb_distance_result), kind, s));
+  if (out->n_unsupported) CK(cudaMemcpyAsync(out->n_unsupported, d_cnt + 3, sizeof(unsigned), kind, s));
+  if (dev) {  // (pageable sources: staged before the call returns)
+    if (out->n_env_candidates) CK(cudaMemcpyAsync(out->n_env_candidates, &n_env, sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    if (out->n_self_candidates) CK(cudaMemcpyAsync(out->n_self_candidates, &n_self, sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    CK(cudaGetLastError());
+    return HFB_OK;
+  }
+  CK(cudaStreamSynchronize(s));
+  if (out->n_env_candidates) *out->n_env_candidates = n_env;
+  if (out->n_self_candidates) *out->n_self_candidates = n_self;
   return HFB_OK;
 }
 
@@ -3315,6 +3432,76 @@ int hfb_env_distance_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32
     CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
                        cudaMemcpyDeviceToDevice, s));
     if (int rc = env_distance_query(ctx, env, n_a, first_a, num_a, req, max_distance, d_out, s, true)) return rc;
+  }
+  // the next call that shares the scratch or this table waits for what is still running here
+  CK(cudaEventRecord(ctx->dev_done, s));
+  ctx->dev_used = true;
+  ctx->dev_last_stream = s;
+  return HFB_OK;
+}
+
+// Each configuration's clearance (hfb_configs_distance_out in include/hppfcl_b200.h): the nearest of its environment
+// pairs (hfb_env_distance's) and its self pairs (the template's), the environment first on ties -- what a planner's
+// clearance(state) is, the smaller of MoveIt's distanceRobot and distanceSelf.
+int hfb_env_distance_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                             size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_config,
+                             size_t num_configs, const hfb_distance_request* req, double max_distance,
+                             const hfb_configs_distance_out* out) {
+  if (!ctx || !env || !req || !configs_distance_ok(out, max_distance) || (n_a && (!handles_a || !tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
+  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
+  for (uint32_t* c : {out->n_env_candidates, out->n_self_candidates, out->n_unsupported})
+    if (c) *c = 0;
+  if (n_a == 0) return HFB_OK;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->slots[0].stream;
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+  const size_t off = env->head - n_a;
+  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
+  CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
+  if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
+  return env_distance_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req,
+                                    max_distance, out, s, false);
+}
+
+int hfb_env_distance_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                    const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                    const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                    const hfb_distance_request* req, double max_distance,
+                                    const hfb_configs_distance_out* d_out, void* stream) {
+  if (!ctx || !env || !req || !configs_distance_ok(d_out, max_distance) || (n_a && (!d_handles_a || !d_tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
+  if (int rc = after_device_calls(ctx, s)) return rc;
+  for (uint32_t* c : {d_out->n_env_candidates, d_out->n_self_candidates, d_out->n_unsupported})
+    if (c) CK(cudaMemsetAsync(c, 0, sizeof(uint32_t), s));
+  if (n_a) {
+    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
+    const size_t off = env->head - n_a;
+    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
+                       cudaMemcpyDeviceToDevice, s));
+    CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
+    if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
+    if (int rc = env_distance_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req,
+                                            max_distance, d_out, s, true))
+      return rc;
   }
   // the next call that shares the scratch or this table waits for what is still running here
   CK(cudaEventRecord(ctx->dev_done, s));

@@ -76,6 +76,9 @@ def load_library(path=None):
     L.hfb_env_distance.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, C.c_double, vp]
     L.hfb_env_distance_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, C.c_double, vp, vp]
     L.hfb_broadphase_config_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, vp, vp, sz, vp]
+    L.hfb_env_distance_configs.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, C.c_double, vp]
+    L.hfb_env_distance_configs_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, C.c_double, vp, vp]
+    L.hfb_broadphase_config_distance_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, C.c_double, vp, vp, sz, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -175,6 +178,32 @@ def broadphase_config_pairs(aabbs, links_per_config, self_pairs, first_config=0,
                                        _ptr(first), _ptr(second), cap, C.byref(cnt))
     if rc != 0:
         raise EngineError("hfb_broadphase_config_pairs: %s" % _ERR.get(rc, rc))
+    k = min(cnt.value, cap)
+    return first[:k], second[:k]
+
+
+def broadphase_config_distance_pairs(aabbs, links_per_config, self_pairs, max_distance=np.inf, first_config=0,
+                                     num_configs=None, capacity=None):
+    """the self pairs whose distance() the configurations distance query runs: boxes (n x 6) of n_configs x
+    links_per_config objects, configuration-major; for every configuration g of [first_config, first_config +
+    num_configs) (default: to the end) and template pair (i, j), (g * L + i, g * L + j) unless both boxes exist and are
+    finite and j's box does not overlap i's box widened by max_distance (rounded outward) -> (first, second),
+    configuration by configuration in template order.  Host function of the library: needs neither a context nor a GPU."""
+    L = load_library()
+    bb = np.ascontiguousarray(aabbs, dtype=np.float64).reshape(-1, 6)
+    tpl = _template(self_pairs)
+    n, lpc = bb.shape[0], int(links_per_config)
+    if num_configs is None:
+        num_configs = max(n // lpc - first_config, 0) if lpc else 0
+    cap = int(capacity) if capacity is not None else max(tpl.shape[0] * int(num_configs), 1)
+    first = np.empty(max(cap, 1), dtype=np.uint32)
+    second = np.empty(max(cap, 1), dtype=np.uint32)
+    cnt = C.c_size_t(0)
+    rc = L.hfb_broadphase_config_distance_pairs(n, _ptr(bb), lpc, tpl.shape[0], _ptr(tpl), int(first_config),
+                                                int(num_configs), float(max_distance), _ptr(first), _ptr(second), cap,
+                                                C.byref(cnt))
+    if rc != 0:
+        raise EngineError("hfb_broadphase_config_distance_pairs: %s" % _ERR.get(rc, rc))
     k = min(cnt.value, cap)
     return first[:k], second[:k]
 
@@ -550,6 +579,51 @@ class Engine:
         self._check(self.L.hfb_env_distance_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a), first_a,
                                                    n_a if num_a is None else num_a, C.byref(req), float(max_distance),
                                                    C.byref(out), _ptr(stream)))
+
+    def env_distance_configs(self, env, handles_a, tfs_a, links_per_config, self_pairs, req=None, max_distance=np.inf,
+                             first_config=0, num_configs=None, records=True):
+        """each configuration's nearest pair, environment or self (hfb_env_distance_configs) -> (kind: 0 environment,
+        1 self, -1 none; first: index in A; second: index in B for kind 0, in A for kind 1, UINT32_MAX for none;
+        min_distance; records or None with records=False; n_env_candidates, n_self_candidates, n_unsupported)"""
+        req = req or P.DistanceRequestPOD()
+        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
+        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
+        if ha.shape[0] != ta.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        tpl = _template(self_pairs)
+        na, lpc = ha.shape[0], int(links_per_config)
+        n_configs = na // lpc if lpc else 0
+        kind = np.empty(n_configs, dtype=np.int8)
+        first = np.empty(n_configs, dtype=np.uint32)
+        second = np.empty(n_configs, dtype=np.uint32)
+        dist = np.empty(n_configs, dtype=np.float64)
+        rec = np.empty(n_configs, dtype=P.distance_result_dtype) if records else None
+        nc = np.zeros(3, dtype=np.uint32)
+        out = P.ConfigsDistanceOut(kind.ctypes.data, first.ctypes.data, second.ctypes.data, dist.ctypes.data,
+                                   None if rec is None else rec.ctypes.data, nc[0:].ctypes.data, nc[1:].ctypes.data,
+                                   nc[2:].ctypes.data)
+        self._check(self.L.hfb_env_distance_configs(self.h, env, na, _ptr(ha), _ptr(ta), lpc, tpl.shape[0], _ptr(tpl),
+                                                    first_config,
+                                                    n_configs - first_config if num_configs is None else num_configs,
+                                                    C.byref(req), float(max_distance), C.byref(out)))
+        return kind, first, second, dist, rec, int(nc[0]), int(nc[1]), int(nc[2])
+
+    def env_distance_configs_device(self, env, n_a, d_handles_a, d_tfs_a, links_per_config, self_pairs, d_kind, d_first,
+                                    d_second, d_min_distance, d_results, d_n_env_candidates=None, d_n_self_candidates=None,
+                                    d_n_unsupported=None, req=None, max_distance=np.inf, stream=0, first_config=0,
+                                    num_configs=None):
+        """hfb_env_distance_configs_device: A's handles and poses and every output are device pointers, ordered on
+        `stream`; the template is a host array"""
+        req = req or P.DistanceRequestPOD()
+        tpl = _template(self_pairs)
+        lpc = int(links_per_config)
+        n_configs = n_a // lpc if lpc else 0
+        out = P.ConfigsDistanceOut(d_kind, d_first, d_second, d_min_distance, d_results, d_n_env_candidates,
+                                   d_n_self_candidates, d_n_unsupported)
+        self._check(self.L.hfb_env_distance_configs_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a), lpc,
+                                                           tpl.shape[0], _ptr(tpl), first_config,
+                                                           n_configs - first_config if num_configs is None else num_configs,
+                                                           C.byref(req), float(max_distance), C.byref(out), _ptr(stream)))
 
     # -- object-table queries: the batched form of the CollisionObject overloads (collision.h:58-61) -----
     @staticmethod

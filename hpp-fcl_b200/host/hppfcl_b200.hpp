@@ -1038,8 +1038,55 @@ class ResidentEnvironment {
     query_distance(robot, request, max_distance, {nullptr, d.data(), nullptr, nullptr, nullptr});
     return d;
   }
+  /// A planner's clearance: per configuration (robot manager laid out as in collide_configurations) its nearest pair
+  /// over the environment pairs and the template's self pairs.  kind[g]: 0 environment, 1 self, -1 none eligible;
+  /// first[g]: index in the robot manager; second[g]: index in the environment (kind 0) or in the robot manager (kind
+  /// 1), UINT32_MAX when none; min_distance[g]: DBL_MAX when none; returns the records.  The eligible pairs and the
+  /// argmin are those of distance(); on a tie an environment pair beats a self pair, and earlier links and template
+  /// entries beat later ones (hfb_env_distance_configs).  A max_distance that is NaN or negative, or a malformed
+  /// template, throws std::invalid_argument.
+  std::vector<hfb_distance_result> distance_configurations(
+      DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+      const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const DistanceRequest& request,
+      std::vector<int8_t>& kind, std::vector<uint32_t>& first, std::vector<uint32_t>& second,
+      std::vector<FCL_REAL>& min_distance, FCL_REAL max_distance = std::numeric_limits<FCL_REAL>::infinity()) {
+    const size_t n = robot_size(robot, max_distance), n_configs = links_per_config ? n / links_per_config : 0;
+    std::vector<hfb_distance_result> rec(n_configs);
+    kind.resize(n_configs);
+    first.resize(n_configs);
+    second.resize(n_configs);
+    min_distance.resize(n_configs);
+    distance_configs(robot, links_per_config, self_pairs, request, max_distance,
+                     {kind.data(), first.data(), second.data(), min_distance.data(), rec.data(), nullptr, nullptr, nullptr});
+    return rec;
+  }
+  /// the distances alone: each configuration's clearance (no records come back)
+  std::vector<FCL_REAL> configuration_clearance(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                                const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                                FCL_REAL max_distance = std::numeric_limits<FCL_REAL>::infinity(),
+                                                const DistanceRequest& request = DistanceRequest()) {
+    const size_t n = robot_size(robot, max_distance);
+    std::vector<FCL_REAL> d(links_per_config ? n / links_per_config : 0);
+    distance_configs(robot, links_per_config, self_pairs, request, max_distance,
+                     {nullptr, nullptr, nullptr, d.data(), nullptr, nullptr, nullptr, nullptr});
+    return d;
+  }
 
  private:
+  void distance_configs(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                        const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const DistanceRequest& request,
+                        FCL_REAL max_distance, const hfb_configs_distance_out& out) {
+    hfb_distance_request q;
+    detail::fill(request, q);
+    std::vector<uint32_t> tpl;
+    for (const auto& p : self_pairs) {
+      tpl.push_back(p.first);
+      tpl.push_back(p.second);
+    }
+    const size_t n_configs = links_per_config ? robot.hs.size() / links_per_config : 0;
+    C.check(hfb_env_distance_configs(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), links_per_config,
+                                     self_pairs.size(), tpl.data(), 0, n_configs, &q, max_distance, &out));
+  }
   size_t robot_size(DynamicAABBTreeCollisionManager& robot, FCL_REAL max_distance) {
     if (!(max_distance >= 0)) throw std::invalid_argument("max_distance must be >= 0 or inf");
     if (robot.stale) robot.refresh();

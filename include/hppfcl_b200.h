@@ -568,6 +568,64 @@ int hfb_broadphase_config_pairs(size_t n_a, const double* aabbs, size_t links_pe
                                 const uint32_t* self_pairs, size_t first_config, size_t num_configs, uint32_t* first,
                                 uint32_t* second, size_t capacity, size_t* n_pairs);
 
+/* ---- a planner's clearance: each configuration's nearest pair, environment or self ---------------------------------
+ * A, the template and the configuration range are laid out and checked as in hfb_env_collide_configs; the distance
+ * rules are those of hfb_env_distance (a fresh DistanceResult per pair; ELIGIBLE: min_distance <= max_distance and not
+ * HFB_PATH_UNSUPPORTED, a NaN distance never is; max_distance >= 0 or +inf, NaN or negative is
+ * HFB_ERR_INVALID_ARGUMENT, checked before the context is read).  For configuration g the pairs are, in this order:
+ *   1. environment pairs (g*L + i, j), j in B: link order first, then B order; each record byte for byte what
+ *      hfb_env_distance returns for that pair;
+ *   2. self pairs (o1 = g*L + i, o2 = g*L + j) in template order; each record byte for byte what
+ *      hfb_batch_distance_objects returns for that pair over the table A.
+ * The winner is the eligible pair with the smallest min_distance (-0.0 == +0.0); on a tie the first in that order, so
+ * an environment pair beats a self pair at the same distance.  This is OMPL's StateValidityChecker::clearance(state),
+ * which MoveIt computes as the smaller of distanceRobot and distanceSelf.  Outputs, n_configs = n_a / L each:
+ *   kind[g]:          0 environment pair, 1 self pair, -1 no eligible pair (int8).
+ *   first[g]:         the winner's index in A; second[g]: its index in B (kind 0) or in A (kind 1); both UINT32_MAX
+ *                     without a winner.
+ *   min_distance[g]:  the winner's distance, DBL_MAX without one; results[g]: its record, a fresh record without one
+ *                     (as hfb_env_distance writes them).  Configurations outside the range get these no-winner values.
+ *   kind, min_distance and results may each be null but not all three; first and second may be null.
+ *   n_env_candidates (may be null): the count hfb_env_distance gives for the range's links; n_self_candidates (may be
+ *   null): the self pairs whose distance() ran; n_unsupported (may be null): pairs of both kinds that came back
+ *   HFB_PATH_UNSUPPORTED.
+ * Environment pairs run as in hfb_env_distance over the range's links.  A self pair is skipped only when both link
+ * boxes exist and are finite and link j's box does not overlap link i's box widened by max_distance, rounded outward
+ * (relying on a box enclosing its shape, as the other calls do); at +inf every template pair runs.  An env with no
+ * objects still checks the self pairs, an empty template still checks the environment.  A refused call writes nothing.
+ * Counts are 32 bits: the self pairs go through the range in chunks of floor((2^32 - 1) / n_self_pairs) configurations.
+ *   hfb_env_distance_configs: HOST buffers, blocking.
+ *   hfb_env_distance_configs_device: A's handles and poses and every output in DEVICE memory, ordered on `cuda_stream`
+ *     (the template stays in host memory).  It blocks on `cuda_stream` where hfb_env_distance_device does (the rounds'
+ *     candidate counts), plus once per chunk of configurations for the self candidate count (once more when they
+ *     outgrow the candidate lists).  Growing a context or env buffer allocates device memory, which waits for the
+ *     whole device.  Later host calls on the context wait for it.
+ *   hfb_broadphase_config_distance_pairs: the self pairs that would run, for boxes `aabbs` (n_a x 6), HOST function, no
+ *     context: configuration by configuration in template order, all counted in *n_pairs, at most `capacity` stored. */
+typedef struct hfb_configs_distance_out {
+  int8_t* kind;
+  uint32_t* first;
+  uint32_t* second;
+  double* min_distance;
+  hfb_distance_result* results;
+  uint32_t* n_env_candidates;
+  uint32_t* n_self_candidates;
+  uint32_t* n_unsupported;
+} hfb_configs_distance_out;
+int hfb_env_distance_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                             size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_config,
+                             size_t num_configs, const hfb_distance_request* req, double max_distance,
+                             const hfb_configs_distance_out* out);
+int hfb_env_distance_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                    const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                    const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                    const hfb_distance_request* req, double max_distance,
+                                    const hfb_configs_distance_out* d_out, void* cuda_stream);
+int hfb_broadphase_config_distance_pairs(size_t n_a, const double* aabbs, size_t links_per_config, size_t n_self_pairs,
+                                         const uint32_t* self_pairs, size_t first_config, size_t num_configs,
+                                         double max_distance, uint32_t* first, uint32_t* second, size_t capacity,
+                                         size_t* n_pairs);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
