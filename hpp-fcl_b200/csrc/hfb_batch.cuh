@@ -24,10 +24,11 @@ struct EpaItem {
 
 // k_epa, tier 0 -> tier 1: a run that filled the reduced-size workspace at the top of an iteration leaves its state
 // here (slot = its position in the retry list) and tier 1 carries on from it in the full-size workspace instead of
-// starting the pair over
+// starting the pair over: the run state, the polytope, and the support points of its vertices (EpaSupArray)
 struct EpaCont {
   EpaResume rs;
-  EpaWsSmall ws;
+  EpaPolySmall ws;
+  double sp[6 * EpaPolySmall::MAXV];
 };
 
 struct BatchArgs {
@@ -50,6 +51,8 @@ struct BatchArgs {
   unsigned* retry_count;
   EpaCont* cont;              // continuation records of the first cont_cap retry positions (null: every retry starts over)
   unsigned cont_cap;
+  double* epa_sup;            // k_epa tier 0: the support points of the polytopes, 6 * EpaPolySmall::MAXV doubles per
+  unsigned epa_sup_groups;    // resident lane group (slot blockIdx.x * GPB + group), for this many groups
   unsigned pair_base;         // added to the pair index of an EPA queue item: the host pipeline runs phase 1 chunk by chunk
                               // (pointers offset to the chunk) and EPA once, over the whole batch (base pointers)
   unsigned sub_idx, sub_cnt;  // k_pairs: this launch takes the sub_idx-th of sub_cnt equal parts of [lo, hi)

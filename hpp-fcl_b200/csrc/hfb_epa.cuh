@@ -41,12 +41,11 @@ namespace hfb {
 #define HFB_EPA_ROUND_FACES 6
 #endif
 
+// the polytope: the vertices' w (w0 - w1), the faces, the walk's scratch
 template <int MAXV_, int MAXF_>
-struct EpaWsT {
+struct EpaPolyT {
   static constexpr int MAXV = MAXV_;
   static constexpr int MAXF = MAXF_;
-  double vw0[MAXV_ * 3];
-  double vw1[MAXV_ * 3];
   double vw[MAXV_ * 3];  // w0 - w1
   double fn[MAXF_ * 3];
   double fd[MAXF_];
@@ -61,12 +60,68 @@ struct EpaWsT {
   uint8_t stk_s[MAXF_ + 4];  // e | stage << 2
   uint8_t newf[MAXF_ + 4];   // faces whose geometry is pending, in creation order
 };
+// the polytope and the vertices' support points w0 / w1, which the loop writes and never reads (a run's side, below)
+template <int MAXV_, int MAXF_>
+struct EpaWsT : EpaPolyT<MAXV_, MAXF_> {
+  double vw0[MAXV_ * 3];
+  double vw1[MAXV_ * 3];
+};
 // full size: any request up to epa_max_iterations = HFB_EPA_CAP_IT fits
 typedef EpaWsT<HFB_EPA_MAXV, HFB_EPA_MAXF> EpaWs;
-// first-try size of the EPA kernel: room for 24 iterations (99% of the penetrating pairs of the
-// benchmark workloads stop within 20), 2.4x more pairs in flight per SM than the full size
+// first-try size of the EPA kernel: room for 24 iterations (99% of the penetrating pairs of the benchmark workloads stop
+// within 20).  k_epa's first tier holds the polytope alone (EpaPolySmall) and keeps the support points of its vertices
+// in a store of their own (EpaSupArray, 6 doubles per vertex, in global memory); EpaWsSmall is the same size with the
+// support points in the workspace, for host callers
 #define HFB_EPA_SMALL_IT 24
+typedef EpaPolyT<HFB_EPA_SMALL_IT + 4, 2 * HFB_EPA_SMALL_IT + 4> EpaPolySmall;
 typedef EpaWsT<HFB_EPA_SMALL_IT + 4, 2 * HFB_EPA_SMALL_IT + 4> EpaWsSmall;
+
+// A run's side: where it keeps what its loop writes and never reads back, the support points w0 / w1 of the polytope's
+// vertices (the witness points read those of the result face's three vertices, the hand-over copies them all).  Every
+// side has:
+//   put<G>(i, sv)             stores w0 / w1 of vertex i
+//   get(i, c), set(i, c, v)   component c of vertex i: w0.x w0.y w0.z w1.x w1.y w1.z
+// EpaSideWs: w0 / w1 in the workspace's own arrays (EpaWsT).
+template <class WS>
+struct EpaSideWs {
+  WS* ws;
+  template <int G>
+  HFB_HD void put(int i, const SV& s) const {
+    ws->vw0[3 * i] = s.w0.x;
+    ws->vw0[3 * i + 1] = s.w0.y;
+    ws->vw0[3 * i + 2] = s.w0.z;
+    ws->vw1[3 * i] = s.w1.x;
+    ws->vw1[3 * i + 1] = s.w1.y;
+    ws->vw1[3 * i + 2] = s.w1.z;
+  }
+  HFB_HD double get(int i, int c) const { return c < 3 ? ws->vw0[3 * i + c] : ws->vw1[3 * i + c - 3]; }
+  HFB_HD void set(int i, int c, double v) const {
+    if (c < 3) ws->vw0[3 * i + c] = v;
+    else ws->vw1[3 * i + c - 3] = v;
+  }
+};
+// EpaSupArray: w0 / w1 in an array of their own, [vertex][w0.x w0.y w0.z w1.x w1.y w1.z].  On the device the G lanes of
+// a group share the six stores of a vertex; on the host (where every lane thread of the lane simulation owns a private
+// copy) one thread makes all six.
+struct EpaSupArray {
+  double* p;
+  template <int G>
+  HFB_HD void put(int i, const SV& s) const {
+#if defined(__CUDA_ARCH__)
+    for (int c = Coop<G>::lane(); c < 6; c += G)
+      p[6 * i + c] = c == 0 ? s.w0.x : c == 1 ? s.w0.y : c == 2 ? s.w0.z : c == 3 ? s.w1.x : c == 4 ? s.w1.y : s.w1.z;
+#else
+    p[6 * i] = s.w0.x;
+    p[6 * i + 1] = s.w0.y;
+    p[6 * i + 2] = s.w0.z;
+    p[6 * i + 3] = s.w1.x;
+    p[6 * i + 4] = s.w1.y;
+    p[6 * i + 5] = s.w1.z;
+#endif
+  }
+  HFB_HD double get(int i, int c) const { return p[6 * i + c]; }
+  HFB_HD void set(int i, int c, double v) const { p[6 * i + c] = v; }
+};
 
 struct EpaParams {
   double tolerance;
@@ -87,14 +142,9 @@ struct EpaState {
 
 template <class WS>
 HFB_HD v3 ws_vw(const WS* ws, int i) { return mk(ws->vw[3 * i], ws->vw[3 * i + 1], ws->vw[3 * i + 2]); }
-template <class WS>
-HFB_HD void ws_put_v(WS* ws, int i, const SV& s) {
-  ws->vw0[3 * i] = s.w0.x;
-  ws->vw0[3 * i + 1] = s.w0.y;
-  ws->vw0[3 * i + 2] = s.w0.z;
-  ws->vw1[3 * i] = s.w1.x;
-  ws->vw1[3 * i + 1] = s.w1.y;
-  ws->vw1[3 * i + 2] = s.w1.z;
+template <int G, class WS, class Side>
+HFB_HD void ws_put_v(WS* ws, const Side& sd, int i, const SV& s) {
+  sd.template put<G>(i, s);
   ws->vw[3 * i] = s.w.x;
   ws->vw[3 * i + 1] = s.w.y;
   ws->vw[3 * i + 2] = s.w.z;
@@ -410,9 +460,9 @@ struct EpaLoop {
 // EPA::evaluate (:1156-1316) in three parts, so that a run which outgrows a reduced-size workspace can continue in the
 // full-size one instead of starting over (k_epa, tier 0 -> tier 1).
 // part 1: encloseOrigin, the initial tetrahedron and its four faces.  False: FallBack (E is final).
-template <int G, int CAPS, class WS>
+template <int G, int CAPS, class WS, class Side>
 HFB_HD bool epa_begin(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const EpaParams& P, GjkState& g, WS* ws,
-                      EpaState& E, EpaLoop& L) {
+                      const Side& sd, EpaState& E, EpaLoop& L) {
   const double tol = P.tolerance;
   E.hint0 = g.hint0;
   E.hint1 = g.hint1;
@@ -438,10 +488,10 @@ HFB_HD bool epa_begin(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const
       g.s0 = g.s1;
       g.s1 = tmp;
     }
-    ws_put_v(ws, 0, g.s0);
-    ws_put_v(ws, 1, g.s1);
-    ws_put_v(ws, 2, g.s2);
-    ws_put_v(ws, 3, g.s3);
+    ws_put_v<G>(ws, sd, 0, g.s0);
+    ws_put_v<G>(ws, sd, 1, g.s1);
+    ws_put_v<G>(ws, sd, 2, g.s2);
+    ws_put_v<G>(ws, sd, 3, g.s3);
     E.num_vertices = 4;
     Coop<G>::sync();  // vertices written above are read by other lanes below
     const int t0 = epa_alloc_face(ws, E, 0, 1, 2);
@@ -475,9 +525,9 @@ HFB_HD bool epa_begin(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const
 
 // part 2: the expansion loop (:1209-1290), from the state (E, L, *ws) -- that of epa_begin, or of an earlier epa_run
 // that stopped with L.resumable set
-template <int G, int CAPS, class WS>
-HFB_HD void epa_run(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const EpaParams& P, WS* ws, EpaState& E,
-                    EpaLoop& L) {
+template <int G, int CAPS, class WS, class Side>
+HFB_HD void epa_run(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const EpaParams& P, WS* ws, const Side& sd,
+                    EpaState& E, EpaLoop& L) {
   const double tol = P.tolerance;
   unsigned it = L.it;
   int pass = L.pass;
@@ -503,7 +553,7 @@ HFB_HD void epa_run(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const E
     ws->fpass[closest] = (uint8_t)(++pass);
     const v3 cn = ws_fn(ws, closest);
     const SV w = gjk_support<G, CAPS>(sa, sb, md, cn, E.hint0, E.hint1);
-    ws_put_v(ws, id_w, w);
+    ws_put_v<G>(ws, sd, id_w, w);
 
     const v3 vf1 = ws_vw(ws, ws->fvid[3 * closest]);
     const v3 vf2 = ws_vw(ws, ws->fvid[3 * closest + 1]);
@@ -549,30 +599,28 @@ HFB_HD void epa_finish(const EpaParams& P, EpaState& E, const EpaLoop& L) {
 }
 HFB_HD double epa_depth(const MinkD& md, const EpaLoop& L) { return L.outer_d + (md.ssr0 + md.ssr1); }
 
-template <int G, int CAPS, class WS>
+template <int G, int CAPS, class WS, class Side>
 HFB_HD void epa_evaluate(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const EpaParams& P, GjkState& g, WS* ws,
-                         EpaState& E, EpaLoop& L) {
-  if (epa_begin<G, CAPS>(sa, sb, md, P, g, ws, E, L)) {
-    epa_run<G, CAPS>(sa, sb, md, P, ws, E, L);
+                         const Side& sd, EpaState& E, EpaLoop& L) {
+  if (epa_begin<G, CAPS>(sa, sb, md, P, g, ws, sd, E, L)) {
+    epa_run<G, CAPS>(sa, sb, md, P, ws, sd, E, L);
     if (!(E.status == HFB_EPA_WS_OVERFLOW && L.resumable)) epa_finish(P, E, L);
   }
 }
 
-// the live part of a workspace copied into a larger one (same slot and vertex numbers), by the G lanes of the group:
-// vertices [0, num_vertices), face slots [0, hwm), the stock of freed slots.  The per-iteration scratch (walk stack,
-// pending faces) is empty at the top of an iteration, which is the only place a run is resumed from.
-template <int G, class WSA, class WSB>
-HFB_HD void epa_ws_grow(const WSA* a, WSB* b, const EpaState& E) {
+// the live part of a workspace (a) and its side (sa) copied into a larger workspace (b) and its side (sb), same slot and
+// vertex numbers, by the G lanes of the group: vertices [0, num_vertices) and their support points, face slots
+// [0, hwm), the stock of freed slots.  The per-iteration scratch (walk stack, pending faces) is empty at the top of an
+// iteration, which is the only place a run is resumed from.
+template <int G, class WSA, class SideA, class WSB, class SideB>
+HFB_HD void epa_ws_grow(const WSA* a, const SideA& sa, WSB* b, const SideB& sb, const EpaState& E) {
 #if !defined(__CUDACC__) && defined(HFB_LANE_SIM)
   const int l = 0, G_ = 1;  // host lane simulation: every lane thread owns private copies of both workspaces
 #else
   const int l = Coop<G>::lane(), G_ = G;
 #endif
-  for (int i = l; i < 3 * E.num_vertices; i += G_) {
-    b->vw0[i] = a->vw0[i];
-    b->vw1[i] = a->vw1[i];
-    b->vw[i] = a->vw[i];
-  }
+  for (int i = l; i < 3 * E.num_vertices; i += G_) b->vw[i] = a->vw[i];
+  for (int i = l; i < 6 * E.num_vertices; i += G_) sb.set(i / 6, i % 6, sa.get(i / 6, i % 6));
   for (int i = l; i < 3 * E.hwm; i += G_) {
     b->fn[i] = a->fn[i];
     b->fvid[i] = a->fvid[i];
@@ -588,25 +636,31 @@ HFB_HD void epa_ws_grow(const WSA* a, WSB* b, const EpaState& E) {
   for (int i = l; i < E.stock_top; i += G_) b->stock[i] = a->stock[i];
   Coop<G>::sync();
 }
+// the same between two workspaces that keep the support points themselves (EpaWsT)
+template <int G, int VA, int FA, int VB, int FB>
+HFB_HD void epa_ws_grow(const EpaWsT<VA, FA>* a, EpaWsT<VB, FB>* b, const EpaState& E) {
+  epa_ws_grow<G>(a, EpaSideWs<const EpaWsT<VA, FA>>{a}, b, EpaSideWs<EpaWsT<VB, FB>>{b}, E);
+}
 
-// the support points of a result vertex, read from the workspace (the store closest_points_inl sums them from; the
+// the support points of a result vertex, read from the run's side (the store closest_points_inl sums them from; the
 // vertex is its w and its id in the workspace)
-template <class WS>
+template <class Side>
 struct WsStore {
   using V = SVSlot;
   static constexpr bool inline_projections = false;
-  const WS* ws;
+  const Side& sd;
   HFB_HD void support_points(const SVSlot& v, v3& w0, v3& w1) const {
-    w0 = mk(ws->vw0[3 * v.slot], ws->vw0[3 * v.slot + 1], ws->vw0[3 * v.slot + 2]);
-    w1 = mk(ws->vw1[3 * v.slot], ws->vw1[3 * v.slot + 1], ws->vw1[3 * v.slot + 2]);
+    w0 = mk(sd.get(v.slot, 0), sd.get(v.slot, 1), sd.get(v.slot, 2));
+    w1 = mk(sd.get(v.slot, 3), sd.get(v.slot, 4), sd.get(v.slot, 5));
   }
 };
 
 // EPA::getWitnessPointsAndNormal (:1451-1466) of a finished run (not FallBack): the result simplex is the closest
-// face's three vertices, read from the workspace where the run left them.  Inlined, with the vertices passed by value:
-// handed by reference to the out-of-line closest_points, they would go through local memory.
-template <class WS>
-HFB_HD void epa_witness(const WS* ws, const EpaLoop& L, double depth, const MinkD& md, v3& w0, v3& w1, v3& normal) {
+// face's three vertices, read from the workspace and the side where the run left them.  Inlined, with the vertices
+// passed by value: handed by reference to the out-of-line closest_points, they would go through local memory.
+template <class WS, class Side>
+HFB_HD void epa_witness(const WS* ws, const Side& sd, const EpaLoop& L, double depth, const MinkD& md, v3& w0, v3& w1,
+                        v3& normal) {
   SVSlot r0, r1, r2;
   r0.w = ws_vw(ws, L.ov0);
   r0.slot = L.ov0;
@@ -614,7 +668,7 @@ HFB_HD void epa_witness(const WS* ws, const EpaLoop& L, double depth, const Mink
   r1.slot = L.ov1;
   r2.w = ws_vw(ws, L.ov2);
   r2.slot = L.ov2;
-  const WsStore<WS> st = {ws};
+  const WsStore<Side> st = {sd};
   closest_points_inl(r0, r1, r2, r0, 3, w0, w1, st);
   if (nrm(w0 - w1) > HFB_DUMMY_PRECISION) {
     if (depth >= 0) normal = unit(w0 - w1);

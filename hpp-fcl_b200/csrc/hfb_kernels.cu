@@ -47,6 +47,8 @@
 #define HFB_GE_DEFAULT 8
 // lanes per pair of the EPA kernel's second tier (k_epa<G,CAPS,MODE,1>), whatever HFB_GE asks for the first
 #define HFB_GE_TIER1 32
+// lane groups per SM the global-memory support-point store of tier 0 is sized for (k_epa; the largest first-tier shape)
+#define HFB_EPA_SUP_GROUPS_PER_SM 64
 
 // pair classes of the device-side counting sort (k_bin_*): bins [0,9) closed-form
 // combos (bin 8: a plane or halfspace against a primitive or another plane), [9,45) GJK-routed
@@ -274,10 +276,12 @@ __global__ void __launch_bounds__(128, 1) k_gjk_refill(const BatchArgs a) {
 }
 
 // ------------------------------------------------------------------ phase 2 --
-// EPA runs in two tiers.  Tier 0 gives every pair a reduced-size workspace (EpaWsSmall), so that 48
-// lane groups fit in one SM's shared memory instead of 20: the kernel is bound by the latency of one
-// pair's dependent FP64 chain, and throughput is the number of pairs in flight.  A pair whose polytope
-// outgrows it is appended to the retry list and run again by tier 1 in the full-size workspace.
+// EPA runs in two tiers.  Tier 0 gives every pair a reduced-size workspace (EpaPolySmall), so that 64 lane groups fit in
+// one SM (4 blocks x 16 groups at 8 lanes per pair) instead of 20: the kernel is bound by the latency of one pair's
+// dependent FP64 chain, and throughput is the number of pairs in flight.  A pair whose polytope outgrows it is appended
+// to the retry list and run again by tier 1 in the full-size workspace.
+// Tier 0 keeps only the polytope in shared memory.  The support points w0 / w1 of its vertices, which the loop writes
+// and never reads, go to global memory (EpaSupArray), one slot per resident lane group: blockIdx.x * GPB + group.
 template <int G, int TIER>
 struct EpaCfg {
   typedef EpaWs WS;
@@ -287,18 +291,28 @@ struct EpaCfg {
 };
 template <int G>
 struct EpaCfg<G, 0> {
-  typedef EpaWsSmall WS;
+  typedef EpaPolySmall WS;
   static constexpr int GPB = (G == 4) ? 24 : ((G == 8) ? 16 : (G == 16 ? 16 : 8));
   static constexpr int THREADS = GPB * G;
-  // G = 8: 3 blocks x 16 groups per SM, 168 registers; G = 4: 2 blocks x 24 groups
-  static constexpr int MINB = (G == 8) ? 3 : (G == 4 ? 2 : 1);
+  // G = 8: 4 blocks x 16 groups per SM at 128 registers (16 warps: 4 per SM sub-partition of 16 K registers); G = 4:
+  // 2 blocks x 24 groups
+  static constexpr int MINB = (G == 8) ? 4 : (G == 4 ? 2 : 1);
 };
+template <int G, int TIER, class WS>
+__device__ __forceinline__ auto epa_side(const BatchArgs& a, WS* ws, unsigned lg) {
+  if constexpr (TIER == 0) {
+    return EpaSupArray{a.epa_sup + (size_t)(blockIdx.x * EpaCfg<G, 0>::GPB + lg) * (6 * WS::MAXV)};
+  } else {
+    return EpaSideWs<WS>{ws};
+  }
+}
 template <int G, int CAPS, int MODE, int TIER>
 __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MINB) k_epa(const BatchArgs a) {
   typedef typename EpaCfg<G, TIER>::WS WS;
   extern __shared__ __align__(16) unsigned char smem[];
   const unsigned lg = threadIdx.x / G;  // group within block
   WS* ws = reinterpret_cast<WS*>(smem) + lg;
+  const auto sd = epa_side<G, TIER>(a, ws, lg);
   const unsigned lo = TIER == 0 ? *a.epa_lo : 0u, hi = TIER == 0 ? *a.epa_hi : *a.retry_count;
   for (;;) {
     unsigned k = 0;
@@ -341,7 +355,7 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
     EpaResume rs;
     bool done;
     if (TIER == 0) {
-      done = pair_epa<G, CAPS>(S, a.P, g, ws, rs);
+      done = pair_epa<G, CAPS>(S, a.P, g, ws, sd, rs);
       if (!done) {
         unsigned r = 0;
         if (Coop<G>::lane() == 0) {
@@ -351,7 +365,10 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
         r = __shfl_sync(Coop<G>::mask(), r, (threadIdx.x & 31u) & ~(unsigned)(G - 1));
         if (a.cont && r < a.cont_cap) {  // (the group's lanes hold the same rs)
           EpaCont* c = a.cont + r;
-          if (rs.L.resumable) epa_ws_grow<G>(ws, &c->ws, rs.E);
+          if (rs.L.resumable) {
+            Coop<G>::sync();  // the support points the other lanes stored
+            epa_ws_grow<G>(ws, sd, &c->ws, EpaSupArray{c->sp}, rs.E);
+          }
           if (Coop<G>::lane() == 0) c->rs = rs;
         }
       }
@@ -359,17 +376,18 @@ __global__ void __launch_bounds__(EpaCfg<G, TIER>::THREADS, EpaCfg<G, TIER>::MIN
       const unsigned kk = k_pos;
       if (a.cont && kk < a.cont_cap && a.cont[kk].rs.L.resumable) {
         rs = a.cont[kk].rs;
-        epa_ws_grow<G>(&a.cont[kk].ws, ws, rs.E);
-        done = pair_epa_resume<G, CAPS>(S, a.P, ws, rs);
+        epa_ws_grow<G>(&a.cont[kk].ws, EpaSupArray{a.cont[kk].sp}, ws, sd, rs.E);
+        done = pair_epa_resume<G, CAPS>(S, a.P, ws, sd, rs);
       } else {
-        done = pair_epa<G, CAPS>(S, a.P, g, ws, rs);
+        done = pair_epa<G, CAPS>(S, a.P, g, ws, sd, rs);
       }
     }
     if (done) {
       // make_setup's tfa: the first pose, or the second one when the operands were swapped (a triangle first)
       S.tfa = load_xf((S.swapped ? a.tf2 : a.tf1)[i].R);
+      if constexpr (TIER == 0) Coop<G>::sync();  // the support points the other lanes stored
       PairOut o;
-      pair_epa_result(S, g.iterations, rs, ws, o);
+      pair_epa_result(S, g.iterations, rs, ws, sd, o);
       if (Coop<G>::lane() == 0) store_result<MODE>(a, i, o);
     }
     Coop<G>::sync();
@@ -830,6 +848,7 @@ struct Slot {
   cudaStream_t work_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_work = nullptr;
   DevBuf cont;  // EpaCont records (k_epa tier 0 -> tier 1)
+  DevBuf sup;   // k_epa tier 0: support points, one slot per resident lane group (a slot runs one tier-0 launch at a time)
   DevBuf h1, h2, tf1, tf2, out, gin, hin, gout, hout, queue, counters, lists, retry, bvh_ws, bvh_cnt, extra, ccnt, okeys, ohist, olist;
   DevBuf qprep, qstacks, qtl, qws, qsv;  // task-system mesh-shape walk (hfb_bvhq.cu)
   DevBuf hsort;                      // hfb_hullsort.cu scratch
@@ -1008,9 +1027,14 @@ int launch_epa(hfb_ctx* ctx, const BatchArgs& a, cudaStream_t s) {
   } else {
     per_sm = it->second;
   }
+  int blocks = ctx->num_sms * per_sm;
+  // tier 0: one support-point slot per resident group (the kernel is grid-persistent: fewer blocks only run longer)
+  if (TIER == 0 && (unsigned)(blocks * EpaCfg<G, TIER>::GPB) > a.epa_sup_groups)
+    blocks = (int)(a.epa_sup_groups / EpaCfg<G, TIER>::GPB);
+  if (blocks < 1) return fail(ctx, HFB_ERR_CUDA, "EPA support-point store missing");
   {
     KTimer kt(ctx, s, 1);
-    k_epa<G, CAPS, MODE, TIER><<<ctx->num_sms * per_sm, threads, smem, s>>>(a);
+    k_epa<G, CAPS, MODE, TIER><<<blocks, threads, smem, s>>>(a);
   }
   ctx->stats.kernel_launches++;
   CK(cudaGetLastError());
@@ -1046,6 +1070,15 @@ int launch_pairs_convex(hfb_ctx* ctx, const BatchArgs& a, unsigned work, cudaStr
     case 16: return launch_pairs<16, CAPS_ALLP, MODE, PATH_BOTH>(ctx, a, work, s);
     default: return launch_pairs<32, CAPS_ALLP, MODE, PATH_BOTH>(ctx, a, work, s);
   }
+}
+
+// the support-point store of k_epa's first tier (one slot per resident lane group) into `a`
+cudaError_t reserve_epa_sup(hfb_ctx* ctx, Slot& sl, BatchArgs& a) {
+  const size_t groups = (size_t)ctx->num_sms * HFB_EPA_SUP_GROUPS_PER_SM;
+  const cudaError_t e = sl.sup.reserve(groups * 6 * EpaPolySmall::MAXV * sizeof(double));
+  a.epa_sup = static_cast<double*>(sl.sup.p);
+  a.epa_sup_groups = e == cudaSuccess ? (unsigned)groups : 0u;
+  return e;
 }
 
 // runs one (sub)batch whose inputs/outputs are already device-resident:
@@ -1088,6 +1121,7 @@ int run_device_batch(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s, int ep
     a.cont = static_cast<EpaCont*>(sl.cont.p);
     a.cont_cap = (unsigned)cap;
   }
+  if (a.P.compute_penetration) CK(reserve_epa_sup(ctx, sl, a));
   unsigned* cnt = static_cast<unsigned*>(sl.counters.p);
   unsigned* mark = cnt + 4;
   unsigned* heads = cnt + 16;
@@ -1360,6 +1394,7 @@ int run_deferred_epa(hfb_ctx* ctx, Slot& sl, BatchArgs a, cudaStream_t s) {
   a.cont = static_cast<EpaCont*>(sl.cont.p);
   a.cont_cap = a.cont ? (unsigned)(((size_t)ctx->epa_resume < (size_t)a.n ? (size_t)ctx->epa_resume : (size_t)a.n)) : 0u;
   if (a.cont && sl.cont.cap < (size_t)a.cont_cap * sizeof(EpaCont)) a.cont_cap = (unsigned)(sl.cont.cap / sizeof(EpaCont));
+  CK(reserve_epa_sup(ctx, sl, a));
   a.A = ctx->dview;
   a.index_list = nullptr;
   a.pair_base = 0;
@@ -1941,7 +1976,7 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   cudaDeviceSynchronize();
   hfb_comm_destroy(c);
   auto rel = [](Slot& s) {
-    DevBuf* bs[] = {&s.h1, &s.h2, &s.tf1, &s.tf2, &s.out, &s.gin, &s.hin, &s.gout, &s.hout, &s.queue, &s.counters, &s.lists, &s.retry, &s.bvh_ws, &s.bvh_cnt, &s.extra, &s.ccnt, &s.okeys, &s.ohist, &s.olist, &s.qprep, &s.qstacks, &s.qtl, &s.qws, &s.qsv, &s.gstate, &s.glist, &s.gcnt, &s.pi, &s.pj, &s.cmp, &s.cont, &s.hsort};
+    DevBuf* bs[] = {&s.h1, &s.h2, &s.tf1, &s.tf2, &s.out, &s.gin, &s.hin, &s.gout, &s.hout, &s.queue, &s.counters, &s.lists, &s.retry, &s.bvh_ws, &s.bvh_cnt, &s.extra, &s.ccnt, &s.okeys, &s.ohist, &s.olist, &s.qprep, &s.qstacks, &s.qtl, &s.qws, &s.qsv, &s.gstate, &s.glist, &s.gcnt, &s.pi, &s.pj, &s.cmp, &s.cont, &s.sup, &s.hsort};
     for (DevBuf* b : bs) b->release();
     if (s.stream) cudaStreamDestroy(s.stream);
     if (s.epa_stream) cudaStreamDestroy(s.epa_stream);

@@ -297,9 +297,11 @@ struct EpaResume {
   EpaState E;
   EpaLoop L;
 };
-// the result record of a finished EPA run (r) whose workspace is `ws`.  Of S it reads the radii, tfa and swapped.
-template <class WS>
-HFB_HD void pair_epa_result(const GjkSetup& S, unsigned gjk_iterations, const EpaResume& r, const WS* ws, PairOut& o) {
+// the result record of a finished EPA run (r) whose workspace is `ws` and side `sd`.  Of S it reads the radii, tfa and
+// swapped.
+template <class WS, class Side>
+HFB_HD void pair_epa_result(const GjkSetup& S, unsigned gjk_iterations, const EpaResume& r, const WS* ws,
+                            const Side& sd, PairOut& o) {
   o.iterations = (gjk_iterations & 0xffffu) | ((r.L.it & 0xffffu) << 16);
   o.status = pack_status(HFB_GJK_COLLISION, r.E.status, HFB_PATH_GJK);
   if (r.E.status == HFB_EPA_FALLBACK) {  // EPAFailedExtract... :713-723
@@ -314,49 +316,63 @@ HFB_HD void pair_epa_result(const GjkSetup& S, unsigned gjk_iterations, const Ep
   o.hint0 = r.E.hint0;
   o.hint1 = r.E.hint1;
   o.distance = fmin(0., -depth);
-  epa_witness(ws, r.L, depth, S.md, o.p1, o.p2, o.normal);
+  epa_witness(ws, sd, r.L, depth, S.md, o.p1, o.p2, o.normal);
   recentre(S.tfa, o.distance, o.p1, o.p2, o.normal);
   unswap(S, o);
 }
 // EPA from GJK's final simplex `g`, up to the result record.  Returns false only when WS is a reduced-size workspace
-// and the polytope outgrew it; with r.L.resumable set, (r, *ws) is then the state at the top of the iteration that did
-// not fit, which pair_epa_resume continues from a copy of (epa_ws_grow); otherwise the pair is run again, from the
+// and the polytope outgrew it; with r.L.resumable set, (r, *ws, sd) is then the state at the top of the iteration that
+// did not fit, which pair_epa_resume continues from a copy of (epa_ws_grow); otherwise the pair is run again, from the
 // queued GJK state, in the full-size workspace.
-template <int G, int CAPS, class WS>
-HFB_HD bool pair_epa(const GjkSetup& S, const SolverP& P, GjkState& g, WS* ws, EpaResume& r) {
-  epa_evaluate<G, CAPS>(S.a, S.b, S.md, P.epa, g, ws, r.E, r.L);
+template <int G, int CAPS, class WS, class Side>
+HFB_HD bool pair_epa(const GjkSetup& S, const SolverP& P, GjkState& g, WS* ws, const Side& sd, EpaResume& r) {
+  epa_evaluate<G, CAPS>(S.a, S.b, S.md, P.epa, g, ws, sd, r.E, r.L);
   return r.E.status != HFB_EPA_WS_OVERFLOW;
 }
-// the rest of a run that stopped with r.L.resumable set; `ws` holds the grown copy of its workspace
-template <int G, int CAPS, class WS>
-HFB_HD bool pair_epa_resume(const GjkSetup& S, const SolverP& P, WS* ws, EpaResume& r) {
-  epa_run<G, CAPS>(S.a, S.b, S.md, P.epa, ws, r.E, r.L);
+// the rest of a run that stopped with r.L.resumable set; `ws` and `sd` hold the grown copy of its workspace and side
+template <int G, int CAPS, class WS, class Side>
+HFB_HD bool pair_epa_resume(const GjkSetup& S, const SolverP& P, WS* ws, const Side& sd, EpaResume& r) {
+  epa_run<G, CAPS>(S.a, S.b, S.md, P.epa, ws, sd, r.E, r.L);
   if (r.E.status == HFB_EPA_WS_OVERFLOW && r.L.resumable) return false;  // (cannot happen in the full-size workspace)
   epa_finish(P.epa, r.E, r.L);
   return r.E.status != HFB_EPA_WS_OVERFLOW;
 }
 // pair_epa + the result record.  Returns false (and leaves `o` unset) only when WS is a reduced-size workspace and the
 // polytope outgrew it; `rs`, if given, then receives the state to resume from (see pair_epa).
-template <int G, int CAPS, class WS>
-HFB_HD bool pair_phase2(const PairIn& in, const SolverP& P, GjkState& g, WS* ws, PairOut& o, EpaResume* rs = nullptr) {
+template <int G, int CAPS, class WS, class Side>
+HFB_HD bool pair_phase2(const PairIn& in, const SolverP& P, GjkState& g, WS* ws, const Side& sd, PairOut& o,
+                        EpaResume* rs = nullptr) {
   GjkSetup S;
   make_setup<CAPS>(in, S);
   EpaResume r;
-  if (!pair_epa<G, CAPS>(S, P, g, ws, r)) {
+  if (!pair_epa<G, CAPS>(S, P, g, ws, sd, r)) {
     if (rs) *rs = r;
     return false;
   }
-  pair_epa_result(S, g.iterations, r, ws, o);
+  pair_epa_result(S, g.iterations, r, ws, sd, o);
   return true;
 }
+// the same in a workspace that keeps the support points itself (EpaWsT)
+template <int G, int CAPS, int V, int F>
+HFB_HD bool pair_phase2(const PairIn& in, const SolverP& P, GjkState& g, EpaWsT<V, F>* ws, PairOut& o,
+                        EpaResume* rs = nullptr) {
+  return pair_phase2<G, CAPS>(in, P, g, ws, EpaSideWs<EpaWsT<V, F>>{ws}, o, rs);
+}
 // pair_epa_resume + the result record; `g` holds the GJK iteration count of the pair (all the record takes from it)
-template <int G, int CAPS, class WS>
-HFB_HD bool pair_phase2_resume(const PairIn& in, const SolverP& P, const GjkState& g, WS* ws, EpaResume& rs, PairOut& o) {
+template <int G, int CAPS, class WS, class Side>
+HFB_HD bool pair_phase2_resume(const PairIn& in, const SolverP& P, const GjkState& g, WS* ws, const Side& sd,
+                               EpaResume& rs, PairOut& o) {
   GjkSetup S;
   make_setup<CAPS>(in, S);
-  if (!pair_epa_resume<G, CAPS>(S, P, ws, rs)) return false;
-  pair_epa_result(S, g.iterations, rs, ws, o);
+  if (!pair_epa_resume<G, CAPS>(S, P, ws, sd, rs)) return false;
+  pair_epa_result(S, g.iterations, rs, ws, sd, o);
   return true;
+}
+// the same in a workspace that keeps the support points itself (EpaWsT)
+template <int G, int CAPS, int V, int F>
+HFB_HD bool pair_phase2_resume(const PairIn& in, const SolverP& P, const GjkState& g, EpaWsT<V, F>* ws, EpaResume& rs,
+                               PairOut& o) {
+  return pair_phase2_resume<G, CAPS>(in, P, g, ws, EpaSideWs<EpaWsT<V, F>>{ws}, rs, o);
 }
 
 // ---- epilogues -----------------------------------------------------------------
