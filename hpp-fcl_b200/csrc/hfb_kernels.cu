@@ -1835,6 +1835,21 @@ int host_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform* 
   return HFB_OK;
 }
 
+// the *_device calls may still be reading the shared scratch (dev_slot, the candidates, their records and counters of
+// hfb_env_collide_device) or an env's table on another stream: a call on stream s that writes them waits for them first
+int after_device_calls(hfb_ctx* ctx, cudaStream_t s) {
+  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
+  if (ctx->dev_used && ctx->dev_last_stream != s) CK(cudaStreamWaitEvent(s, ctx->dev_done, 0));
+  return HFB_OK;
+}
+// the device call on s is the last one: the next call on another stream waits for what is still running here
+int last_device_call(hfb_ctx* ctx, cudaStream_t s) {
+  ctx->dev_used = true;
+  ctx->dev_last_stream = s;
+  CK(cudaEventRecord(ctx->dev_done, s));
+  return HFB_OK;
+}
+
 template <int MODE, typename Req>
 int device_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform* tf1, const uint32_t* h2,
                  const hfb_transform* tf2, const Req* req, const SolverP& P, const CollideP& Cp, const BvhReq& Bq,
@@ -1861,12 +1876,9 @@ int device_batch(hfb_ctx* ctx, size_t n, const uint32_t* h1, const hfb_transform
   a.guess_out = go ? go->cached_gjk_guess : nullptr;
   a.hint_out = go ? go->cached_support_func_guess : nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (ctx->dev_used && ctx->dev_last_stream != st) CK(cudaStreamWaitEvent(st, ctx->dev_done, 0));
+  if ((rc = after_device_calls(ctx, st))) return rc;
   rc = run_device_batch<MODE>(ctx, ctx->dev_slot, a, st);
-  ctx->dev_used = true;
-  ctx->dev_last_stream = st;
-  CK(cudaEventRecord(ctx->dev_done, st));
+  if (int e = last_device_call(ctx, st)) return e;
   return rc;
 }
 
@@ -2410,9 +2422,8 @@ static int objects_device(hfb_ctx* ctx, const hfb_object_pairs* sc, const Req* r
   if (!sc->object_handles || !sc->object_tfs || !sc->first || !sc->second || !out) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "null buffer");
   CK(cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (ctx->dev_used && ctx->dev_last_stream != st) CK(cudaStreamWaitEvent(st, ctx->dev_done, 0));
-  ctx->dev_used = true;  // (the expansion below already writes the shared scratch)
+  if (int rc = after_device_calls(ctx, st)) return rc;
+  ctx->dev_used = true;  // (the expansion below already writes the shared scratch; device_batch records the event)
   ctx->dev_last_stream = st;
   Slot& sl = ctx->dev_slot;
   CK(sl.h1.reserve(n * 4));
@@ -2513,12 +2524,6 @@ int hfb_broadphase_pairs_device(hfb_ctx* ctx, size_t n, const double* d_aabbs, s
 
 }  // extern "C"
 
-// the *_device calls may still be reading the shared scratch (the candidates, their records and counters of
-// hfb_env_collide_device) or an env's table on another stream: a call on stream s that writes them waits for them first
-static int after_device_calls(hfb_ctx* ctx, cudaStream_t s) {
-  if (ctx->dev_used && ctx->dev_last_stream != s) CK(cudaStreamWaitEvent(s, ctx->dev_done, 0));
-  return HFB_OK;
-}
 // The number of candidate pairs is not known in advance: find(cap, &launches) launches a pair finder that counts every
 // candidate in the counter's first word (d_cnt) and stores at most `cap` in each of `lists` (4 bytes per candidate).
 // find_all runs it and reads the counter's first n_words words into `words`; when the count exceeded the lists, they
@@ -2583,12 +2588,63 @@ static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32
                            nullptr, s);
 }
 
+// Where a query's outputs go, on stream s.  Host form (dev false): the caller's outputs are host memory; device results
+// are downloaded, and the counts the host knows are written once finish() has waited for the downloads.  Device form:
+// they are device memory, written in stream order, and finish() does not wait.
+struct QueryOut {
+  cudaStream_t s;
+  bool dev;
+  bool pending = false;                                // host form: downloads not waited for yet
+  std::vector<std::pair<uint32_t*, unsigned>> counts;  // host form: written by finish()
+
+  cudaError_t zero(void* p, size_t bytes) {
+    if (!p || !bytes) return cudaSuccess;
+    if (dev) return cudaMemsetAsync(p, 0, bytes, s);
+    std::memset(p, 0, bytes);
+    return cudaSuccess;
+  }
+  // `bytes` of device memory at src into dst
+  cudaError_t copy(void* dst, const void* src, size_t bytes) {
+    if (!dst) return cudaSuccess;
+    pending |= !dev;
+    return cudaMemcpyAsync(dst, src, bytes, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s);
+  }
+  // the first `width` bytes of each of n records of `pitch` bytes at src (a field, such as the records' min_distance),
+  // packed into dst
+  cudaError_t copy_field(void* dst, const void* src, size_t width, size_t pitch, size_t n) {
+    if (!dst) return cudaSuccess;
+    pending |= !dev;
+    return cudaMemcpy2DAsync(dst, width, src, pitch, width, n, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s);
+  }
+  // a count the host knows; the device form copies it from d_v when the device holds it there, else from the host
+  // (pageable source: staged before the call returns)
+  cudaError_t count(uint32_t* dst, unsigned v, const unsigned* d_v = nullptr) {
+    if (!dst) return cudaSuccess;
+    if (!dev) {
+      counts.emplace_back(dst, v);
+      return cudaSuccess;
+    }
+    if (d_v) return cudaMemcpyAsync(dst, d_v, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
+    return cudaMemcpyAsync(dst, &v, sizeof(unsigned), cudaMemcpyHostToDevice, s);
+  }
+  cudaError_t finish() {
+    if (dev) return cudaGetLastError();
+    if (pending) {
+      if (cudaError_t e = cudaStreamSynchronize(s)) return e;
+      pending = false;
+    }
+    for (const auto& c : counts) *c.first = c.second;
+    counts.clear();
+    return cudaSuccess;
+  }
+};
+
 // The colliding ones of scene_candidates' `cand` candidates: compacted (pairs and records, at most out->capacity; not
-// when out->flags is set and capacity is 0) and flagged per A object (out->flags, n_flags of them, when set).  dev: the
-// outputs are device memory, written on s; else host memory, downloaded.  `second_base` is subtracted from the second
-// indices.
-static int scene_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, uint32_t second_base, const hfb_env_out* out,
-                        size_t n_flags, bool dev) {
+// when out->flags is set and capacity is 0) and flagged per A object (out->flags, n_flags of them, when set), then
+// o.finish().  `second_base` is subtracted from the second indices.
+static int scene_output(hfb_ctx* ctx, unsigned cand, uint32_t second_base, const hfb_env_out* out, size_t n_flags,
+                        QueryOut& o) {
+  const cudaStream_t s = o.s;
   unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
   const hfb_contact* recs = static_cast<const hfb_contact*>(ctx->sc_out.p);
   const uint32_t* pf = static_cast<const uint32_t*>(ctx->sc_pf.p);
@@ -2596,7 +2652,7 @@ static int scene_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, uint32_t se
   CK(cudaMemsetAsync(d_cnt + 1, 0, sizeof(unsigned), s));
   uint8_t* flags = out->flags;
   if (flags) {
-    if (!dev) {
+    if (!o.dev) {  // (the host form stages its outputs in the scratch)
       CK(ctx->sc_flags.reserve(n_flags));
       flags = static_cast<uint8_t*>(ctx->sc_flags.p);
     }
@@ -2607,7 +2663,7 @@ static int scene_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, uint32_t se
   uint32_t *first = out->first, *second = out->second;
   hfb_contact* contacts = out->contacts;
   if (compact) {
-    if (!dev) {
+    if (!o.dev) {
       CK(ctx->sc_f.reserve((size_t)out->capacity * 4 + 4));
       CK(ctx->sc_s.reserve((size_t)out->capacity * 4 + 4));
       CK(ctx->sc_rec.reserve((size_t)out->capacity * sizeof(hfb_contact) + 8));
@@ -2619,28 +2675,29 @@ static int scene_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, uint32_t se
                                                         first, second, contacts, out->capacity);
     ctx->stats.kernel_launches++;
   }
-  if (dev) {
+  if (o.dev) {
     const unsigned most = cand < out->capacity ? cand : out->capacity;
     if (compact && second_base && most) {
       k_unbase<<<(most + 255) / 256, 256, 0, s>>>(out->second, d_cnt + 1, out->capacity, second_base);
       ctx->stats.kernel_launches++;
     }
-    if (out->n_colliding) CK(cudaMemcpyAsync(out->n_colliding, d_cnt + 1, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
-    CK(cudaGetLastError());
+    CK(o.copy(out->n_colliding, d_cnt + 1, sizeof(unsigned)));
+    CK(o.finish());
     return HFB_OK;
   }
+  // the host form sizes the download by the count
   unsigned hits = 0;
   CK(cudaMemcpyAsync(&hits, d_cnt + 1, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (out->n_colliding) *out->n_colliding = hits;
+  CK(o.count(out->n_colliding, hits));
   const unsigned kept = !compact ? 0u : hits < out->capacity ? hits : out->capacity;
   if (kept) {
-    CK(cudaMemcpyAsync(out->first, first, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(out->second, second, (size_t)kept * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(out->contacts, contacts, (size_t)kept * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
+    CK(o.copy(out->first, first, (size_t)kept * 4));
+    CK(o.copy(out->second, second, (size_t)kept * 4));
+    CK(o.copy(out->contacts, contacts, (size_t)kept * sizeof(hfb_contact)));
   }
-  if (flags) CK(cudaMemcpyAsync(out->flags, flags, n_flags, cudaMemcpyDeviceToHost, s));
-  if (kept || flags) CK(cudaStreamSynchronize(s));
+  if (flags) CK(o.copy(out->flags, flags, n_flags));
+  CK(o.finish());
   if (second_base)
     for (unsigned k = 0; k < kept; ++k) out->second[k] -= second_base;
   return HFB_OK;
@@ -2656,8 +2713,9 @@ static int scene_collide_table(hfb_ctx* ctx, cudaStream_t s, size_t n, const uin
   if (int rc = scene_candidates(ctx, s, n, d_h, d_tf, n, find_pairs, req, minus_inf, &cand)) return rc;
   if (out->n_candidates) *out->n_candidates = cand;
   if (cand == 0 || minus_inf) return HFB_OK;
-  const hfb_env_out o{out->first, out->second, out->contacts, out->capacity, out->n_colliding, nullptr, nullptr};
-  return scene_output(ctx, s, cand, second_base, &o, 0, false);
+  const hfb_env_out eo{out->first, out->second, out->contacts, out->capacity, out->n_colliding, nullptr, nullptr};
+  QueryOut o{s, false};
+  return scene_output(ctx, cand, second_base, &eo, 0, o);
 }
 
 extern "C" {
@@ -2859,33 +2917,58 @@ static int env_build(hfb_ctx* ctx, hfb_env* e, cudaStream_t s) {
   ctx->stats.kernel_launches += (uint64_t)nl;
   return HFB_OK;
 }
-// one query of A (already in the table in front of B) against the env: boxes of A, the candidates against the built
-// grid, the narrow phase, then the outputs (host or device)
-static int env_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a, const hfb_collision_request* req,
-                     bool minus_inf, const hfb_env_out* out, cudaStream_t s, bool dev) {
-  const size_t n_b = e->n_b, a_hi = first_a + (num_a < n_a ? num_a : n_a);
-  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
-  const double* bb_b = static_cast<const double*>(e->bb.p);
-  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
-  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
-    if (int rc = bp_cross_query_reset(g, d_cnt, s)) return rc;
-    return bp_cross_query_launch(n_a, d_bb, first_a, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt, ctx->bp_scratch.p,
-                                 ctx->num_sms, s, nl);
-  };
-  const size_t off = e->head - n_a;
-  unsigned cand = 0;
-  if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
-                                static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand))
-    return rc;
-  if (out->n_candidates) {
-    if (dev)
-      CK(cudaMemcpyAsync(out->n_candidates, ctx->sc_cnt.p, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
-    else
-      *out->n_candidates = cand;
+// the configurations of a query: A is configurations of `links` objects each, the range is [g0, g0 + ng), and the
+// template lists the n self pairs (link i, link j) of a configuration
+struct ConfigTpl {
+  size_t links, n;
+  const uint32_t* pairs;
+  size_t g0, ng;
+};
+
+// The queries of an env, each run in env_call's frame: check() is the query's own check of the request, under the
+// lock; zero(o) zeroes its outputs; empty(): nothing to compute, the outputs stay zero; run(o): the query of A
+// (already in the table in front of B) against the env, then its outputs and o.finish().
+
+// hfb_env_collide: boxes of A, the candidates against the built grid, the narrow phase, then the outputs
+struct EnvCollide {
+  const hfb_collision_request* req;
+  const hfb_env_out* out;
+  size_t first_a, num_a;
+  bool minus_inf = false;
+
+  const ConfigTpl* tpl() const { return nullptr; }
+  int check(hfb_ctx* ctx) { return collide_prelude(ctx, req, &minus_inf); }
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t n_a) const {
+    CK(o.zero(out->n_candidates, sizeof(uint32_t)));
+    CK(o.zero(out->n_colliding, sizeof(uint32_t)));
+    CK(o.zero(out->flags, n_a));
+    return HFB_OK;
   }
-  if (cand == 0 || minus_inf) return HFB_OK;
-  return scene_output(ctx, s, cand, (uint32_t)n_a, out, n_a, dev);
-}
+  bool empty(const hfb_env* e, size_t n_a) const { return n_a == 0 || e->n_b == 0; }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const size_t n_b = e->n_b, a_hi = first_a + (num_a < n_a ? num_a : n_a);
+    const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+    const double* bb_b = static_cast<const double*>(e->bb.p);
+    CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+    auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+      if (int rc = bp_cross_query_reset(g, d_cnt, s)) return rc;
+      return bp_cross_query_launch(n_a, d_bb, first_a, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
+                                   ctx->bp_scratch.p, ctx->num_sms, s, nl);
+    };
+    const size_t off = e->head - n_a;
+    unsigned cand = 0;
+    if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
+                                  static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand))
+      return rc;
+    CK(o.count(out->n_candidates, cand, static_cast<const unsigned*>(ctx->sc_cnt.p)));
+    if (cand == 0 || minus_inf) {
+      CK(o.finish());
+      return HFB_OK;
+    }
+    return scene_output(ctx, cand, (uint32_t)n_a, out, n_a, o);
+  }
+};
 
 // hfb_env_collide_configs' arguments beyond the pointers: the layout of A, the configuration range and the template
 static int configs_args(hfb_ctx* ctx, size_t n_a, size_t links, size_t n_tpl, const uint32_t* tpl, size_t g0, size_t ng) {
@@ -2899,9 +2982,10 @@ static bool contacts_ok(const hfb_scene_contacts& o) { return !o.capacity || (o.
 
 // The outputs of hfb_env_collide_configs from the `cand` candidates, the environment pairs before `split`, the self
 // pairs from there on: verdicts per configuration, and each kind compacted into its own outputs with its own counter
-// (sc_cnt[1], sc_cnt[2]).  dev / host outputs as in scene_output.
-static int configs_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, unsigned split, uint32_t second_base, size_t links,
-                          size_t n_configs, const hfb_configs_out* out, bool dev) {
+// (sc_cnt[1], sc_cnt[2]), then o.finish(), as in scene_output.
+static int configs_output(hfb_ctx* ctx, unsigned cand, unsigned split, uint32_t second_base, size_t links,
+                          size_t n_configs, const hfb_configs_out* out, QueryOut& o) {
+  const cudaStream_t s = o.s;
   unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
   const hfb_contact* recs = static_cast<const hfb_contact*>(ctx->sc_out.p);
   const uint32_t* pf = static_cast<const uint32_t*>(ctx->sc_pf.p);
@@ -2910,7 +2994,7 @@ static int configs_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, unsigned 
   CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
   uint8_t* verdicts = out->verdicts;
   if (verdicts) {
-    if (!dev) {
+    if (!o.dev) {  // (the host form stages its outputs in the scratch)
       CK(ctx->sc_flags.reserve(n_configs));
       verdicts = static_cast<uint8_t*>(ctx->sc_flags.p);
     }
@@ -2923,7 +3007,7 @@ static int configs_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, unsigned 
   const unsigned lo[2] = {0, split}, num[2] = {split, cand - split};
   uint32_t *first[2], *second[2];
   hfb_contact* contacts[2];
-  if (!dev) {  // both kinds staged in one set of buffers, the self pairs after the environment's
+  if (!o.dev) {  // both kinds staged in one set of buffers, the self pairs after the environment's
     const size_t total = (size_t)out->env.capacity + out->self.capacity;
     CK(ctx->sc_f.reserve(total * 4 + 4));
     CK(ctx->sc_s.reserve(total * 4 + 4));
@@ -2931,85 +3015,99 @@ static int configs_output(hfb_ctx* ctx, cudaStream_t s, unsigned cand, unsigned 
   }
   for (int k = 0; k < 2; ++k) {
     const size_t at = k ? out->env.capacity : 0;
-    first[k] = dev ? kinds[k]->first : static_cast<uint32_t*>(ctx->sc_f.p) + at;
-    second[k] = dev ? kinds[k]->second : static_cast<uint32_t*>(ctx->sc_s.p) + at;
-    contacts[k] = dev ? kinds[k]->contacts : static_cast<hfb_contact*>(ctx->sc_rec.p) + at;
+    first[k] = o.dev ? kinds[k]->first : static_cast<uint32_t*>(ctx->sc_f.p) + at;
+    second[k] = o.dev ? kinds[k]->second : static_cast<uint32_t*>(ctx->sc_s.p) + at;
+    contacts[k] = o.dev ? kinds[k]->contacts : static_cast<hfb_contact*>(ctx->sc_rec.p) + at;
     if (!compact || num[k] == 0) continue;
     k_compact_scene<<<(num[k] + 255) / 256, 256, 0, s>>>(recs + lo[k], pf + lo[k], ps + lo[k], num[k], d_cnt + 1 + k,
                                                           first[k], second[k], contacts[k], kinds[k]->capacity);
     ctx->stats.kernel_launches++;
   }
-  if (dev) {
+  if (o.dev) {
     const unsigned most = split < out->env.capacity ? split : out->env.capacity;
     if (compact && most) {  // (only the environment's second indices are in B)
       k_unbase<<<(most + 255) / 256, 256, 0, s>>>(out->env.second, d_cnt + 1, out->env.capacity, second_base);
       ctx->stats.kernel_launches++;
     }
-    for (int k = 0; k < 2; ++k)
-      if (kinds[k]->n_colliding)
-        CK(cudaMemcpyAsync(kinds[k]->n_colliding, d_cnt + 1 + k, sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
-    CK(cudaGetLastError());
+    for (int k = 0; k < 2; ++k) CK(o.copy(kinds[k]->n_colliding, d_cnt + 1 + k, sizeof(unsigned)));
+    CK(o.finish());
     return HFB_OK;
   }
+  // the host form sizes the downloads by the counts
   unsigned hits[2] = {0, 0}, kept[2];
   CK(cudaMemcpyAsync(hits, d_cnt + 1, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   for (int k = 0; k < 2; ++k) {
-    if (kinds[k]->n_colliding) *kinds[k]->n_colliding = hits[k];
+    CK(o.count(kinds[k]->n_colliding, hits[k]));
     kept[k] = !compact ? 0u : hits[k] < kinds[k]->capacity ? hits[k] : kinds[k]->capacity;
     if (!kept[k]) continue;
-    CK(cudaMemcpyAsync(kinds[k]->first, first[k], (size_t)kept[k] * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(kinds[k]->second, second[k], (size_t)kept[k] * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(kinds[k]->contacts, contacts[k], (size_t)kept[k] * sizeof(hfb_contact), cudaMemcpyDeviceToHost, s));
+    CK(o.copy(kinds[k]->first, first[k], (size_t)kept[k] * 4));
+    CK(o.copy(kinds[k]->second, second[k], (size_t)kept[k] * 4));
+    CK(o.copy(kinds[k]->contacts, contacts[k], (size_t)kept[k] * sizeof(hfb_contact)));
   }
-  if (verdicts) CK(cudaMemcpyAsync(out->verdicts, verdicts, n_configs, cudaMemcpyDeviceToHost, s));
-  if (kept[0] || kept[1] || verdicts) CK(cudaStreamSynchronize(s));
+  if (verdicts) CK(o.copy(out->verdicts, verdicts, n_configs));
+  CK(o.finish());
   for (unsigned k = 0; k < kept[0]; ++k) out->env.second[k] -= second_base;
   return HFB_OK;
 }
 
-// one configurations query of A (already in the table in front of B, the template in ctx->sc_tpl): one candidate
-// list -- the environment pairs against the built grid, then, after the split is noted in the counter's second word,
-// the self pairs appended to it -- one narrow phase over the table [A; B], then the outputs (host or device)
-static int env_configs_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t links, size_t n_tpl, size_t g0, size_t ng,
-                             const hfb_collision_request* req, bool minus_inf, const hfb_configs_out* out, cudaStream_t s,
-                             bool dev) {
-  const size_t n_b = e->n_b, a_lo = g0 * links, a_hi = (g0 + ng) * links;
-  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
-  const double* bb_b = static_cast<const double*>(e->bb.p);
-  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
-  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
-  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
-    int rc = 0;
-    if (n_b) {
-      rc = bp_cross_query_reset(g, d_cnt, s);
-      if (!rc)
-        rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt, ctx->bp_scratch.p,
-                                   ctx->num_sms, s, nl);
-    } else {
-      rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
+// hfb_env_collide_configs (the template in ctx->sc_tpl): one candidate list -- the environment pairs against the
+// built grid, then, after the split is noted in the counter's second word, the self pairs appended to it -- one narrow
+// phase over the table [A; B], then the outputs
+struct EnvCollideConfigs {
+  const hfb_collision_request* req;
+  const hfb_configs_out* out;
+  ConfigTpl t;
+  bool minus_inf = false;
+
+  const ConfigTpl* tpl() const { return &t; }
+  int check(hfb_ctx* ctx) { return collide_prelude(ctx, req, &minus_inf); }
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t n_a) const {
+    for (const hfb_scene_contacts* k : {&out->env, &out->self}) {
+      CK(o.zero(k->n_candidates, sizeof(uint32_t)));
+      CK(o.zero(k->n_colliding, sizeof(uint32_t)));
     }
-    if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
-    if (!rc) rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
-    return rc;
-  };
-  const size_t off = e->head - n_a;
-  unsigned cand = 0, split = 0;
-  if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
-                                static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand, &split))
-    return rc;
-  const unsigned n_cand[2] = {split, cand - split};
-  const hfb_scene_contacts* kinds[2] = {&out->env, &out->self};
-  for (int k = 0; k < 2; ++k) {
-    if (!kinds[k]->n_candidates) continue;
-    if (dev)  // (pageable source: staged before the call returns)
-      CK(cudaMemcpyAsync(kinds[k]->n_candidates, &n_cand[k], sizeof(unsigned), cudaMemcpyHostToDevice, s));
-    else
-      *kinds[k]->n_candidates = n_cand[k];
+    CK(o.zero(out->verdicts, n_a / t.links));
+    return HFB_OK;
   }
-  if (cand == 0 || minus_inf) return HFB_OK;
-  return configs_output(ctx, s, cand, split, (uint32_t)n_a, links, n_a / links, out, dev);
-}
+  bool empty(const hfb_env* e, size_t n_a) const { return n_a == 0 || t.ng == 0 || (e->n_b == 0 && t.n == 0); }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const size_t n_b = e->n_b, links = t.links, n_tpl = t.n, g0 = t.g0, ng = t.ng;
+    const size_t a_lo = g0 * links, a_hi = (g0 + ng) * links;
+    const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+    const double* bb_b = static_cast<const double*>(e->bb.p);
+    const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+    CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+    auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+      int rc = 0;
+      if (n_b) {
+        rc = bp_cross_query_reset(g, d_cnt, s);
+        if (!rc)
+          rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
+                                     ctx->bp_scratch.p, ctx->num_sms, s, nl);
+      } else {
+        rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
+      }
+      if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
+      if (!rc) rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
+      return rc;
+    };
+    const size_t off = e->head - n_a;
+    unsigned cand = 0, split = 0;
+    if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
+                                  static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand,
+                                  &split))
+      return rc;
+    CK(o.count(out->env.n_candidates, split));
+    CK(o.count(out->self.n_candidates, cand - split));
+    if (cand == 0 || minus_inf) {
+      CK(o.finish());
+      return HFB_OK;
+    }
+    return configs_output(ctx, cand, split, (uint32_t)n_a, links, n_a / links, out, o);
+  }
+};
 
 // hfb_env_distance's output and cutoff (max_distance >= 0 or +inf), checked before the context is looked at
 static bool env_distance_ok(const hfb_env_distance_out* o, double max_distance) {
@@ -3098,114 +3196,173 @@ static int env_distance_rounds(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t a_lo
   return HFB_OK;
 }
 
-// one distance query of A against the env: the rounds over the range, then the per-A outputs (host or device)
-static int env_distance_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t first_a, size_t num_a,
-                              const hfb_distance_request* req, double maxd, const hfb_env_distance_out* out, cudaStream_t s,
-                              bool dev) {
-  const size_t a_lo = first_a < n_a ? first_a : n_a, a_hi = a_lo + (num_a < n_a - a_lo ? num_a : n_a - a_lo);
-  BpDistState st;
-  unsigned n_cand = 0;
-  if (int rc = env_distance_rounds(ctx, e, n_a, a_lo, a_hi, req, maxd, s, &st, &n_cand)) return rc;
-  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
-  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  if (out->nearest) CK(cudaMemcpyAsync(out->nearest, st.nearest, n_a * 4, kind, s));
-  if (out->min_distance)  // (the records' first field)
-    CK(cudaMemcpy2DAsync(out->min_distance, sizeof(double), st.rec, sizeof(hfb_distance_result), sizeof(double), n_a, kind, s));
-  if (out->results) CK(cudaMemcpyAsync(out->results, st.rec, n_a * sizeof(hfb_distance_result), kind, s));
-  if (out->n_unsupported) CK(cudaMemcpyAsync(out->n_unsupported, d_cnt + 3, sizeof(unsigned), kind, s));
-  if (dev) {
-    if (out->n_candidates)  // (pageable source: staged before the call returns)
-      CK(cudaMemcpyAsync(out->n_candidates, &n_cand, sizeof(unsigned), cudaMemcpyHostToDevice, s));
-    CK(cudaGetLastError());
+// hfb_env_distance: the rounds over the range, then the per-A outputs
+struct EnvDistance {
+  const hfb_distance_request* req;
+  double maxd;
+  const hfb_env_distance_out* out;
+  size_t first_a, num_a;
+
+  const ConfigTpl* tpl() const { return nullptr; }
+  int check(hfb_ctx* ctx) const {
+    if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
     return HFB_OK;
   }
-  CK(cudaStreamSynchronize(s));
-  if (out->n_candidates) *out->n_candidates = n_cand;
-  return HFB_OK;
-}
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t) const {
+    CK(o.zero(out->n_candidates, sizeof(uint32_t)));
+    CK(o.zero(out->n_unsupported, sizeof(uint32_t)));
+    return HFB_OK;
+  }
+  bool empty(const hfb_env*, size_t n_a) const { return n_a == 0; }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const size_t a_lo = first_a < n_a ? first_a : n_a, a_hi = a_lo + (num_a < n_a - a_lo ? num_a : n_a - a_lo);
+    BpDistState st;
+    unsigned n_cand = 0;
+    if (int rc = env_distance_rounds(ctx, e, n_a, a_lo, a_hi, req, maxd, o.s, &st, &n_cand)) return rc;
+    const unsigned* d_cnt = static_cast<const unsigned*>(ctx->sc_cnt.p);
+    CK(o.copy(out->nearest, st.nearest, n_a * 4));
+    CK(o.copy_field(out->min_distance, st.rec, sizeof(double), sizeof(hfb_distance_result), n_a));  // (the first field)
+    CK(o.copy(out->results, st.rec, n_a * sizeof(hfb_distance_result)));
+    CK(o.copy(out->n_unsupported, d_cnt + 3, sizeof(unsigned)));
+    CK(o.count(out->n_candidates, n_cand));
+    CK(o.finish());
+    return HFB_OK;
+  }
+};
 
 // hfb_env_distance_configs' output and cutoff, checked before the context is looked at
 static bool configs_distance_ok(const hfb_configs_distance_out* o, double max_distance) {
   return o && (o->kind || o->min_distance || o->results) && max_distance >= 0;
 }
 
-// one configurations distance query of A (already in the table in front of B, the template in ctx->sc_tpl): the rounds
-// over the range's links, then per chunk of configurations the self pairs config_dist_pair runs, distance() of them
-// over the table [A; B], and the winner of each configuration from its links' winners and its self records (in
-// ctx->sc_cdist).  Blocks for the self candidate count once per chunk (and once more when the lists grow).  Then the
-// outputs (host or device).
-static int env_distance_configs_query(hfb_ctx* ctx, hfb_env* e, size_t n_a, size_t links, size_t n_tpl, size_t g0,
-                                      size_t ng, const hfb_distance_request* req, double maxd,
-                                      const hfb_configs_distance_out* out, cudaStream_t s, bool dev) {
-  const size_t n_b = e->n_b, n_configs = n_a / links;
-  BpDistState st;
-  unsigned n_env = 0;
-  if (int rc = env_distance_rounds(ctx, e, n_a, g0 * links, (g0 + ng) * links, req, maxd, s, &st, &n_env)) return rc;
-  CK(ctx->sc_cdist.reserve(bp_config_dist_bytes(n_configs)));
-  const BpConfigDist cs = bp_config_dist_carve(ctx->sc_cdist.p, n_configs);
-  const size_t off = e->head - n_a;
-  const double* d_ba = static_cast<const double*>(ctx->sc_bb.p);  // (A's boxes, from the rounds)
-  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
-  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
-  int nl = 0;
-  if (bp_config_dist_init_launch(n_configs, cs, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_cfg_init launch failed");
-  uint64_t total = 0;
-  // the self candidates are counted in 32 bits: chunks of configurations whose template entries number fewer than 2^32
-  // (whole configurations, so that each chunk's winners are final)
-  const size_t chunk = n_tpl ? 0xffffffffull / n_tpl : (ng ? ng : 1);
-  for (size_t c0 = g0; c0 < g0 + ng; c0 += chunk) {
-    const size_t c1 = g0 + ng - c0 > chunk ? c0 + chunk : g0 + ng;
-    unsigned kept = 0;
-    if (n_tpl) {
-      auto find = [&](size_t cap, int* launches) {
-        return bp_config_dist_pairs_launch(d_ba, links, d_tpl, n_tpl, c0, c1 - c0, maxd, static_cast<uint32_t*>(ctx->sc_pf.p),
-                                           static_cast<uint32_t*>(ctx->sc_ps.p), static_cast<uint32_t*>(ctx->sc_f.p), cap,
-                                           d_cnt, ctx->num_sms, s, launches);
-      };
-      unsigned words[1] = {0};
-      if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps, &ctx->sc_f}, d_cnt, find, words, 1)) return rc;
-      kept = words[0];
-      total += kept;
-    }
-    if (kept) {
-      CK(ctx->sc_drec.reserve((size_t)kept * sizeof(hfb_distance_result)));
-      hfb_object_pairs sc;
-      sc.n_objects = n_a + n_b;
-      sc.object_handles = static_cast<const uint32_t*>(e->h.p) + off;
-      sc.object_tfs = static_cast<const hfb_transform*>(e->tf.p) + off;
-      sc.n_pairs = kept;
-      sc.first = static_cast<const uint32_t*>(ctx->sc_pf.p);
-      sc.second = static_cast<const uint32_t*>(ctx->sc_ps.p);
-      if (int rc = objects_device<0>(ctx, &sc, req, solver_from_distance_request(*req), CollideP{0, 0},
-                                     bvh_req_of_distance(req), ctx->sc_drec.p, nullptr, s))
-        return rc;
-    }
-    if (bp_config_dist_reduce_launch(st, c0 * links, c1 * links, links, static_cast<const hfb_distance_result*>(ctx->sc_drec.p),
-                                     static_cast<const uint32_t*>(ctx->sc_pf.p), static_cast<const uint32_t*>(ctx->sc_ps.p),
-                                     static_cast<const uint32_t*>(ctx->sc_f.p), kept, maxd, cs, d_cnt + 3, s, &nl) != 0)
-      return fail(ctx, HFB_ERR_CUDA, "k_cfg_min launch failed");
-  }
-  ctx->stats.kernel_launches += (uint64_t)nl;
-  const unsigned n_self = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
-  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  if (out->kind) CK(cudaMemcpyAsync(out->kind, cs.kind, n_configs, kind, s));
-  if (out->first) CK(cudaMemcpyAsync(out->first, cs.first, n_configs * 4, kind, s));
-  if (out->second) CK(cudaMemcpyAsync(out->second, cs.second, n_configs * 4, kind, s));
-  if (out->min_distance)  // (the records' first field)
-    CK(cudaMemcpy2DAsync(out->min_distance, sizeof(double), cs.rec, sizeof(hfb_distance_result), sizeof(double), n_configs,
-                         kind, s));
-  if (out->results) CK(cudaMemcpyAsync(out->results, cs.rec, n_configs * sizeof(hfb_distance_result), kind, s));
-  if (out->n_unsupported) CK(cudaMemcpyAsync(out->n_unsupported, d_cnt + 3, sizeof(unsigned), kind, s));
-  if (dev) {  // (pageable sources: staged before the call returns)
-    if (out->n_env_candidates) CK(cudaMemcpyAsync(out->n_env_candidates, &n_env, sizeof(unsigned), cudaMemcpyHostToDevice, s));
-    if (out->n_self_candidates) CK(cudaMemcpyAsync(out->n_self_candidates, &n_self, sizeof(unsigned), cudaMemcpyHostToDevice, s));
-    CK(cudaGetLastError());
+// hfb_env_distance_configs (the template in ctx->sc_tpl): the rounds over the range's links, then per chunk of
+// configurations the self pairs config_dist_pair runs, distance() of them over the table [A; B], and the winner of
+// each configuration from its links' winners and its self records (in ctx->sc_cdist).  Blocks for the self candidate
+// count once per chunk (and once more when the lists grow).  Then the outputs.
+struct EnvDistanceConfigs {
+  const hfb_distance_request* req;
+  double maxd;
+  const hfb_configs_distance_out* out;
+  ConfigTpl t;
+
+  const ConfigTpl* tpl() const { return &t; }
+  int check(hfb_ctx* ctx) const {
+    if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
     return HFB_OK;
   }
-  CK(cudaStreamSynchronize(s));
-  if (out->n_env_candidates) *out->n_env_candidates = n_env;
-  if (out->n_self_candidates) *out->n_self_candidates = n_self;
-  return HFB_OK;
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t) const {
+    for (uint32_t* c : {out->n_env_candidates, out->n_self_candidates, out->n_unsupported})
+      CK(o.zero(c, sizeof(uint32_t)));
+    return HFB_OK;
+  }
+  bool empty(const hfb_env*, size_t n_a) const { return n_a == 0; }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const size_t n_b = e->n_b, links = t.links, n_tpl = t.n, g0 = t.g0, ng = t.ng, n_configs = n_a / links;
+    BpDistState st;
+    unsigned n_env = 0;
+    if (int rc = env_distance_rounds(ctx, e, n_a, g0 * links, (g0 + ng) * links, req, maxd, s, &st, &n_env)) return rc;
+    CK(ctx->sc_cdist.reserve(bp_config_dist_bytes(n_configs)));
+    const BpConfigDist cs = bp_config_dist_carve(ctx->sc_cdist.p, n_configs);
+    const size_t off = e->head - n_a;
+    const double* d_ba = static_cast<const double*>(ctx->sc_bb.p);  // (A's boxes, from the rounds)
+    unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+    const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+    int nl = 0;
+    if (bp_config_dist_init_launch(n_configs, cs, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_cfg_init launch failed");
+    uint64_t total = 0;
+    // the self candidates are counted in 32 bits: chunks of configurations whose template entries number fewer than
+    // 2^32 (whole configurations, so that each chunk's winners are final)
+    const size_t chunk = n_tpl ? 0xffffffffull / n_tpl : (ng ? ng : 1);
+    for (size_t c0 = g0; c0 < g0 + ng; c0 += chunk) {
+      const size_t c1 = g0 + ng - c0 > chunk ? c0 + chunk : g0 + ng;
+      unsigned kept = 0;
+      if (n_tpl) {
+        auto find = [&](size_t cap, int* launches) {
+          return bp_config_dist_pairs_launch(d_ba, links, d_tpl, n_tpl, c0, c1 - c0, maxd,
+                                             static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p),
+                                             static_cast<uint32_t*>(ctx->sc_f.p), cap, d_cnt, ctx->num_sms, s, launches);
+        };
+        unsigned words[1] = {0};
+        if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps, &ctx->sc_f}, d_cnt, find, words, 1)) return rc;
+        kept = words[0];
+        total += kept;
+      }
+      if (kept) {
+        CK(ctx->sc_drec.reserve((size_t)kept * sizeof(hfb_distance_result)));
+        hfb_object_pairs sc;
+        sc.n_objects = n_a + n_b;
+        sc.object_handles = static_cast<const uint32_t*>(e->h.p) + off;
+        sc.object_tfs = static_cast<const hfb_transform*>(e->tf.p) + off;
+        sc.n_pairs = kept;
+        sc.first = static_cast<const uint32_t*>(ctx->sc_pf.p);
+        sc.second = static_cast<const uint32_t*>(ctx->sc_ps.p);
+        if (int rc = objects_device<0>(ctx, &sc, req, solver_from_distance_request(*req), CollideP{0, 0},
+                                       bvh_req_of_distance(req), ctx->sc_drec.p, nullptr, s))
+          return rc;
+      }
+      if (bp_config_dist_reduce_launch(st, c0 * links, c1 * links, links,
+                                       static_cast<const hfb_distance_result*>(ctx->sc_drec.p),
+                                       static_cast<const uint32_t*>(ctx->sc_pf.p), static_cast<const uint32_t*>(ctx->sc_ps.p),
+                                       static_cast<const uint32_t*>(ctx->sc_f.p), kept, maxd, cs, d_cnt + 3, s, &nl) != 0)
+        return fail(ctx, HFB_ERR_CUDA, "k_cfg_min launch failed");
+    }
+    ctx->stats.kernel_launches += (uint64_t)nl;
+    const unsigned n_self = total > 0xffffffffull ? 0xffffffffu : (unsigned)total;
+    CK(o.copy(out->kind, cs.kind, n_configs));
+    CK(o.copy(out->first, cs.first, n_configs * 4));
+    CK(o.copy(out->second, cs.second, n_configs * 4));
+    CK(o.copy_field(out->min_distance, cs.rec, sizeof(double), sizeof(hfb_distance_result), n_configs));  // (the first field)
+    CK(o.copy(out->results, cs.rec, n_configs * sizeof(hfb_distance_result)));
+    CK(o.copy(out->n_unsupported, d_cnt + 3, sizeof(unsigned)));
+    CK(o.count(out->n_env_candidates, n_env));
+    CK(o.count(out->n_self_candidates, n_self));
+    CK(o.finish());
+    return HFB_OK;
+  }
+};
+
+// The frame of the hfb_env_* queries (EnvCollide, EnvCollideConfigs, EnvDistance, EnvDistanceConfigs), with their
+// pointers checked: the lock, the query's and the env's checks, A uploaded into the env's table in front of B (and
+// the template `tpl` of a configurations query into ctx->sc_tpl), then the query.  Host form (Form::host): A and the
+// outputs are host memory, the call runs on the context's first stream and blocks, and it returns before the device
+// when there is no work.  Device form: they are device memory, the call is ordered on `stream` and records the
+// context's device event.
+enum class Form { host, device };
+template <class Query>
+static int env_call(hfb_ctx* ctx, hfb_env* env, Form form, void* stream, size_t n_a, const uint32_t* h_a,
+                    const hfb_transform* tf_a, Query q) {
+  const bool dev = form == Form::device;
+  const ConfigTpl* tpl = q.tpl();
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (int rc = q.check(ctx)) return rc;
+  if (int rc = env_ready(ctx, env)) return rc;
+  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
+  if (tpl)
+    if (int rc = configs_args(ctx, n_a, tpl->links, tpl->n, tpl->pairs, tpl->g0, tpl->ng)) return rc;
+  QueryOut o{dev ? static_cast<cudaStream_t>(stream) : ctx->slots[0].stream, dev};
+  if (!dev) {
+    if (int rc = check_handles(ctx, h_a, n_a)) return rc;
+    if (int rc = q.zero(ctx, o, n_a)) return rc;
+    if (q.empty(env, n_a)) return HFB_OK;
+  }
+  CK(cudaSetDevice(ctx->device));
+  if (int rc = after_device_calls(ctx, o.s)) return rc;
+  if (dev) {
+    if (int rc = q.zero(ctx, o, n_a)) return rc;
+    if (q.empty(env, n_a)) return last_device_call(ctx, o.s);
+  }
+  if (int rc = env_make_room(ctx, env, n_a, o.s)) return rc;
+  const size_t off = env->head - n_a;
+  const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, h_a, n_a * 4, kind, o.s));
+  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tf_a, n_a * sizeof(hfb_transform), kind, o.s));
+  if (tpl) {
+    CK(ctx->sc_tpl.reserve(tpl->n * 8 + 8));
+    if (tpl->n) CK(cudaMemcpyAsync(ctx->sc_tpl.p, tpl->pairs, tpl->n * 8, cudaMemcpyHostToDevice, o.s));
+  }
+  if (int rc = q.run(ctx, env, n_a, o)) return rc;
+  return dev ? last_device_call(ctx, o.s) : HFB_OK;
 }
 
 extern "C" {
@@ -3274,24 +3431,7 @@ int hfb_env_collide(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* hand
                     size_t first_a, size_t num_a, const hfb_collision_request* req, const hfb_env_out* out) {
   if (!ctx || !env || !req || !out || (n_a && (!handles_a || !tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
   if (out->capacity && (!out->first || !out->second || !out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  bool minus_inf;
-  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
-  if (out->n_candidates) *out->n_candidates = 0;
-  if (out->n_colliding) *out->n_colliding = 0;
-  if (out->flags && n_a) std::memset(out->flags, 0, n_a);
-  if (n_a == 0 || env->n_b == 0) return HFB_OK;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->slots[0].stream;
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-  const size_t off = env->head - n_a;
-  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
-  return env_query(ctx, env, n_a, first_a, num_a, req, minus_inf, out, s, false);
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a, EnvCollide{req, out, first_a, num_a});
 }
 
 int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a, const hfb_transform* d_tfs_a,
@@ -3299,31 +3439,7 @@ int hfb_env_collide_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_
                            void* stream) {
   if (!ctx || !env || !req || !d_out || (n_a && (!d_handles_a || !d_tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
   if (d_out->capacity && (!d_out->first || !d_out->second || !d_out->contacts)) return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  bool minus_inf;
-  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (d_out->n_candidates) CK(cudaMemsetAsync(d_out->n_candidates, 0, sizeof(uint32_t), s));
-  if (d_out->n_colliding) CK(cudaMemsetAsync(d_out->n_colliding, 0, sizeof(uint32_t), s));
-  if (d_out->flags && n_a) CK(cudaMemsetAsync(d_out->flags, 0, n_a, s));
-  if (n_a && env->n_b) {
-    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-    const size_t off = env->head - n_a;
-    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
-                       cudaMemcpyDeviceToDevice, s));
-    if (int rc = env_query(ctx, env, n_a, first_a, num_a, req, minus_inf, d_out, s, true)) return rc;
-  }
-  // the next call that shares the scratch or this table waits for what is still running here
-  CK(cudaEventRecord(ctx->dev_done, s));
-  ctx->dev_used = true;
-  ctx->dev_last_stream = s;
-  return HFB_OK;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a, EnvCollide{req, d_out, first_a, num_a});
 }
 
 int hfb_env_destroy(hfb_ctx* ctx, hfb_env* env) {
@@ -3352,30 +3468,8 @@ int hfb_env_collide_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32
   if (!ctx || !env || !req || !out || (n_a && (!handles_a || !tfs_a)) || (n_self_pairs && !self_pairs))
     return HFB_ERR_INVALID_ARGUMENT;
   if (!contacts_ok(out->env) || !contacts_ok(out->self)) return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  bool minus_inf;
-  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
-  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
-  for (const hfb_scene_contacts* o : {&out->env, &out->self}) {
-    if (o->n_candidates) *o->n_candidates = 0;
-    if (o->n_colliding) *o->n_colliding = 0;
-  }
-  if (out->verdicts && n_a) std::memset(out->verdicts, 0, n_a / links_per_config);
-  if (n_a == 0 || num_configs == 0 || (env->n_b == 0 && n_self_pairs == 0)) return HFB_OK;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->slots[0].stream;
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-  const size_t off = env->head - n_a;
-  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
-  CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
-  if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
-  return env_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req, minus_inf, out, s,
-                           false);
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a,
+                  EnvCollideConfigs{req, out, {links_per_config, n_self_pairs, self_pairs, first_config, num_configs}});
 }
 
 int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
@@ -3385,38 +3479,8 @@ int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
   if (!ctx || !env || !req || !d_out || (n_a && (!d_handles_a || !d_tfs_a)) || (n_self_pairs && !self_pairs))
     return HFB_ERR_INVALID_ARGUMENT;
   if (!contacts_ok(d_out->env) || !contacts_ok(d_out->self)) return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  bool minus_inf;
-  if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  for (const hfb_scene_contacts* o : {&d_out->env, &d_out->self}) {
-    if (o->n_candidates) CK(cudaMemsetAsync(o->n_candidates, 0, sizeof(uint32_t), s));
-    if (o->n_colliding) CK(cudaMemsetAsync(o->n_colliding, 0, sizeof(uint32_t), s));
-  }
-  if (d_out->verdicts && n_a) CK(cudaMemsetAsync(d_out->verdicts, 0, n_a / links_per_config, s));
-  if (n_a && num_configs && (env->n_b || n_self_pairs)) {
-    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-    const size_t off = env->head - n_a;
-    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
-                       cudaMemcpyDeviceToDevice, s));
-    CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
-    if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
-    if (int rc = env_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req, minus_inf,
-                                   d_out, s, true))
-      return rc;
-  }
-  // the next call that shares the scratch or this table waits for what is still running here
-  CK(cudaEventRecord(ctx->dev_done, s));
-  ctx->dev_used = true;
-  ctx->dev_last_stream = s;
-  return HFB_OK;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
+                  EnvCollideConfigs{req, d_out, {links_per_config, n_self_pairs, self_pairs, first_config, num_configs}});
 }
 
 // Each A object's nearest B object (hfb_env_distance_out in include/hppfcl_b200.h): the result of
@@ -3427,22 +3491,8 @@ int hfb_env_distance(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* han
                      size_t first_a, size_t num_a, const hfb_distance_request* req, double max_distance,
                      const hfb_env_distance_out* out) {
   if (!ctx || !env || !req || !env_distance_ok(out, max_distance) || (n_a && (!handles_a || !tfs_a))) return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
-  if (out->n_candidates) *out->n_candidates = 0;
-  if (out->n_unsupported) *out->n_unsupported = 0;
-  if (n_a == 0) return HFB_OK;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->slots[0].stream;
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-  const size_t off = env->head - n_a;
-  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
-  return env_distance_query(ctx, env, n_a, first_a, num_a, req, max_distance, out, s, false);
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a,
+                  EnvDistance{req, max_distance, out, first_a, num_a});
 }
 
 int hfb_env_distance_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a, const hfb_transform* d_tfs_a,
@@ -3450,29 +3500,8 @@ int hfb_env_distance_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32
                             const hfb_env_distance_out* d_out, void* stream) {
   if (!ctx || !env || !req || !env_distance_ok(d_out, max_distance) || (n_a && (!d_handles_a || !d_tfs_a)))
     return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (d_out->n_candidates) CK(cudaMemsetAsync(d_out->n_candidates, 0, sizeof(uint32_t), s));
-  if (d_out->n_unsupported) CK(cudaMemsetAsync(d_out->n_unsupported, 0, sizeof(uint32_t), s));
-  if (n_a) {
-    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-    const size_t off = env->head - n_a;
-    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
-                       cudaMemcpyDeviceToDevice, s));
-    if (int rc = env_distance_query(ctx, env, n_a, first_a, num_a, req, max_distance, d_out, s, true)) return rc;
-  }
-  // the next call that shares the scratch or this table waits for what is still running here
-  CK(cudaEventRecord(ctx->dev_done, s));
-  ctx->dev_used = true;
-  ctx->dev_last_stream = s;
-  return HFB_OK;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
+                  EnvDistance{req, max_distance, d_out, first_a, num_a});
 }
 
 // Each configuration's clearance (hfb_configs_distance_out in include/hppfcl_b200.h): the nearest of its environment
@@ -3485,26 +3514,8 @@ int hfb_env_distance_configs(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint3
   if (!ctx || !env || !req || !configs_distance_ok(out, max_distance) || (n_a && (!handles_a || !tfs_a)) ||
       (n_self_pairs && !self_pairs))
     return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
-  if (int rc = check_handles(ctx, handles_a, n_a)) return rc;
-  for (uint32_t* c : {out->n_env_candidates, out->n_self_candidates, out->n_unsupported})
-    if (c) *c = 0;
-  if (n_a == 0) return HFB_OK;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->slots[0].stream;
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-  const size_t off = env->head - n_a;
-  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, handles_a, n_a * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tfs_a, n_a * sizeof(hfb_transform), cudaMemcpyHostToDevice, s));
-  CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
-  if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
-  return env_distance_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req,
-                                    max_distance, out, s, false);
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a,
+                  EnvDistanceConfigs{req, max_distance, out, {links_per_config, n_self_pairs, self_pairs, first_config, num_configs}});
 }
 
 int hfb_env_distance_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
@@ -3515,34 +3526,8 @@ int hfb_env_distance_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, cons
   if (!ctx || !env || !req || !configs_distance_ok(d_out, max_distance) || (n_a && (!d_handles_a || !d_tfs_a)) ||
       (n_self_pairs && !self_pairs))
     return HFB_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  if (int rc = validate_query(req->q)) return fail(ctx, rc, "invalid request");
-  if (int rc = env_ready(ctx, env)) return rc;
-  if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (int rc = configs_args(ctx, n_a, links_per_config, n_self_pairs, self_pairs, first_config, num_configs)) return rc;
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!ctx->dev_done) CK(cudaEventCreateWithFlags(&ctx->dev_done, cudaEventDisableTiming));
-  if (int rc = after_device_calls(ctx, s)) return rc;
-  for (uint32_t* c : {d_out->n_env_candidates, d_out->n_self_candidates, d_out->n_unsupported})
-    if (c) CK(cudaMemsetAsync(c, 0, sizeof(uint32_t), s));
-  if (n_a) {
-    if (int rc = env_make_room(ctx, env, n_a, s)) return rc;
-    const size_t off = env->head - n_a;
-    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, d_handles_a, n_a * 4, cudaMemcpyDeviceToDevice, s));
-    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, d_tfs_a, n_a * sizeof(hfb_transform),
-                       cudaMemcpyDeviceToDevice, s));
-    CK(ctx->sc_tpl.reserve(n_self_pairs * 8 + 8));
-    if (n_self_pairs) CK(cudaMemcpyAsync(ctx->sc_tpl.p, self_pairs, n_self_pairs * 8, cudaMemcpyHostToDevice, s));
-    if (int rc = env_distance_configs_query(ctx, env, n_a, links_per_config, n_self_pairs, first_config, num_configs, req,
-                                            max_distance, d_out, s, true))
-      return rc;
-  }
-  // the next call that shares the scratch or this table waits for what is still running here
-  CK(cudaEventRecord(ctx->dev_done, s));
-  ctx->dev_used = true;
-  ctx->dev_last_stream = s;
-  return HFB_OK;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
+                  EnvDistanceConfigs{req, max_distance, d_out, {links_per_config, n_self_pairs, self_pairs, first_config, num_configs}});
 }
 
 int hfb_batch_convex_support_device(hfb_ctx* ctx, size_t n, const uint32_t* ids, const double* dirs,

@@ -434,12 +434,8 @@ class Engine:
         """broadphase + narrow phase of set A against set B in one call (hfb_scene_collide_sets)
         -> (first = index in A, second = index in B, contacts, n_candidates, n_colliding), in no particular order"""
         req = req or P.CollisionRequestPOD()
-        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
-        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
-        hb = np.ascontiguousarray(handles_b, dtype=np.uint32)
-        tb = np.ascontiguousarray(tfs_b, dtype=P.transform_dtype)
-        if ha.shape[0] != ta.shape[0] or hb.shape[0] != tb.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        ha, ta = self._objects(handles_a, tfs_a)
+        hb, tb = self._objects(handles_b, tfs_b)
         na, nb = ha.shape[0], hb.shape[0]
         cap = int(capacity) if capacity is not None else max(4 * (na + nb), 1024)
         if bufs is None:
@@ -455,10 +451,7 @@ class Engine:
     # -- resident environment (hfb_env_*): set B's table, boxes and grid kept on the device across queries -------
     def env_create(self, handles_b, tfs_b):
         """set B on the device (its boxes as of now and the cross grid over them) -> an opaque env handle"""
-        hb = np.ascontiguousarray(handles_b, dtype=np.uint32)
-        tb = np.ascontiguousarray(tfs_b, dtype=P.transform_dtype)
-        if hb.shape[0] != tb.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        hb, tb = self._objects(handles_b, tfs_b)
         env = C.c_void_p()
         self._check(self.L.hfb_env_create(self.h, hb.shape[0], _ptr(hb), _ptr(tb), C.byref(env)))
         return env
@@ -476,10 +469,7 @@ class Engine:
         index in B, contacts, n_candidates, n_colliding), plus one flag byte per A object (1: it collides) with
         flags=True.  capacity=0 with flags=True: no pair records at all"""
         req = req or P.CollisionRequestPOD()
-        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
-        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
-        if ha.shape[0] != ta.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        ha, ta = self._objects(handles_a, tfs_a)
         na = ha.shape[0]
         cap = int(capacity) if capacity is not None else max(4 * na, 1024)
         if bufs is None:
@@ -514,10 +504,7 @@ class Engine:
         n_colliding); self = (first, second: indices in A, contacts, n_candidates, n_colliding)).  Both capacities 0 with
         verdicts=True: no pair records at all"""
         req = req or P.CollisionRequestPOD()
-        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
-        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
-        if ha.shape[0] != ta.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        ha, ta = self._objects(handles_a, tfs_a)
         tpl = _template(self_pairs)
         na, lpc = ha.shape[0], int(links_per_config)
         n_configs = na // lpc if lpc else 0
@@ -556,10 +543,7 @@ class Engine:
         """each A object's nearest B object (hfb_env_distance) -> (nearest: index in B or -1, min_distance, records or
         None with records=False, n_candidates, n_unsupported)"""
         req = req or P.DistanceRequestPOD()
-        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
-        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
-        if ha.shape[0] != ta.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        ha, ta = self._objects(handles_a, tfs_a)
         na = ha.shape[0]
         nearest = np.empty(na, dtype=np.int32)
         dist = np.empty(na, dtype=np.float64)
@@ -586,10 +570,7 @@ class Engine:
         1 self, -1 none; first: index in A; second: index in B for kind 0, in A for kind 1, UINT32_MAX for none;
         min_distance; records or None with records=False; n_env_candidates, n_self_candidates, n_unsupported)"""
         req = req or P.DistanceRequestPOD()
-        ha = np.ascontiguousarray(handles_a, dtype=np.uint32)
-        ta = np.ascontiguousarray(tfs_a, dtype=P.transform_dtype)
-        if ha.shape[0] != ta.shape[0]:
-            raise ValueError("handle and pose arrays must have equal length")
+        ha, ta = self._objects(handles_a, tfs_a)
         tpl = _template(self_pairs)
         na, lpc = ha.shape[0], int(links_per_config)
         n_configs = na // lpc if lpc else 0
@@ -624,6 +605,15 @@ class Engine:
                                                            tpl.shape[0], _ptr(tpl), first_config,
                                                            n_configs - first_config if num_configs is None else num_configs,
                                                            C.byref(req), float(max_distance), C.byref(out), _ptr(stream)))
+
+    @staticmethod
+    def _objects(handles, tfs):
+        """an object set as the C ABI takes it: handles and poses, contiguous and of equal length"""
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        t = np.ascontiguousarray(tfs, dtype=P.transform_dtype)
+        if h.shape[0] != t.shape[0]:
+            raise ValueError("handle and pose arrays must have equal length")
+        return h, t
 
     # -- object-table queries: the batched form of the CollisionObject overloads (collision.h:58-61) -----
     @staticmethod
