@@ -173,6 +173,12 @@ class ConfigsDistanceOut(C.Structure):  # hfb_configs_distance_out: per configur
                 ("n_unsupported", C.c_void_p)]
 
 
+class MotionsOut(C.Structure):  # hfb_motions_out: per motion its first colliding sample and the first pair colliding there
+    _fields_ = [("first_invalid", C.c_void_p), ("kind", C.c_void_p), ("first", C.c_void_p), ("second", C.c_void_p),
+                ("contacts", C.c_void_p), ("n_env_candidates", C.c_void_p), ("n_env_colliding", C.c_void_p),
+                ("n_self_candidates", C.c_void_p), ("n_self_colliding", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

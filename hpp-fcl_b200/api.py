@@ -755,6 +755,56 @@ class ResidentEnvironment:
         return self.engine.env_distance_configs(self._env, h, t, links_per_config, tpl, req, max_distance,
                                                 records=False)[3]
 
+    def collide_motions(self, robot_manager, links_per_config, self_pairs, motion_offsets, request=None, first_motion=0,
+                        num_motions=None):
+        """A planner's motion validation: the robot manager holds configurations laid out as in
+        collide_configurations(), the samples of each motion one after another in walking order; motion m is
+        configurations [motion_offsets[m], motion_offsets[m+1]).  -> per motion (first_invalid: the first sample that
+        collides with the environment or with itself, -1 when none does; kind: 0 environment pair, 1 self pair, -1 none;
+        first: index in the robot manager; second: index in the environment for kind 0, in the robot manager for kind 1;
+        contacts: the pair's contact record).  The pair is the first colliding one of that sample: environment pairs by
+        link, then by environment index, then self pairs in template order (include/hppfcl_b200.h,
+        hfb_env_collide_motions).  Only motions [first_motion, first_motion + num_motions) are checked; the others
+        get the no-witness values."""
+        h, t, req = self._robot(robot_manager, request)
+        tpl = self._template_args(links_per_config, self_pairs)
+        off, first_motion, num_motions = self._motion_args(len(h), links_per_config, motion_offsets, first_motion,
+                                                           num_motions)
+        return self.engine.env_collide_motions(self._env, h, t, links_per_config, tpl, off, req, first_motion,
+                                               num_motions)[:5]
+
+    def first_invalid_samples(self, robot_manager, links_per_config, self_pairs, motion_offsets, request=None,
+                              first_motion=0, num_motions=None):
+        """-> first_invalid of collide_motions() alone (no pair records come back)"""
+        h, t, req = self._robot(robot_manager, request)
+        tpl = self._template_args(links_per_config, self_pairs)
+        off, first_motion, num_motions = self._motion_args(len(h), links_per_config, motion_offsets, first_motion,
+                                                           num_motions)
+        return self.engine.env_collide_motions(self._env, h, t, links_per_config, tpl, off, req, first_motion,
+                                               num_motions, witness=False)[0]
+
+    @staticmethod
+    def _motion_args(n_objects, links_per_config, motion_offsets, first_motion, num_motions):
+        """the offsets and the motion range as the C ABI takes them; ones the C ABI refuses raise ValueError (the C++
+        mirror throws std::invalid_argument)"""
+        off = np.asarray(motion_offsets, dtype=np.int64).reshape(-1)
+        lpc = int(links_per_config)
+        if lpc < 1 or n_objects % lpc:
+            raise ValueError("the robot manager's size is not a multiple of links_per_config")
+        if off.shape[0] == 0 or off[0] != 0:
+            raise ValueError("motion offsets must start at 0")
+        if (np.diff(off) < 0).any():
+            raise ValueError("motion offsets decrease")
+        if off[-1] != n_objects // lpc:
+            raise ValueError("motion offsets must end at the number of configurations")
+        if (np.diff(off) > 0x7fffffff).any():
+            raise ValueError("a motion has more than INT32_MAX samples")
+        n_motions = off.shape[0] - 1
+        num_motions = n_motions - first_motion if num_motions is None else num_motions
+        if first_motion < 0 or num_motions < 0 or first_motion + num_motions > n_motions:
+            raise ValueError("motion range past the end")
+        return off.astype(np.uint32), int(first_motion), int(num_motions)
+
     @staticmethod
     def _template_args(links_per_config, self_pairs):
         """the template as the C ABI takes it; one the C ABI refuses raises ValueError (the C++ mirror throws

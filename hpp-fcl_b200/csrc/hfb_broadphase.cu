@@ -419,6 +419,32 @@ __global__ void __launch_bounds__(128) k_config_pairs(const double* bb, unsigned
   }
 }
 
+// k_config_pairs with each pair's template entry in `entry` at its position in the list (hfb_env_collide_motions' tie
+// order)
+__global__ void __launch_bounds__(128) k_config_entry_pairs(const double* bb, unsigned links, const uint32_t* tpl,
+                                                            unsigned n_tpl, unsigned g0, size_t total, uint32_t* first,
+                                                            uint32_t* second, uint32_t* entry, unsigned capacity,
+                                                            unsigned* n_pairs) {
+  const size_t tend = (total + 31u) & ~(size_t)31;  // (warp-uniform trip count for the ballots)
+  const unsigned lane = threadIdx.x & 31u;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < tend; t += (size_t)gridDim.x * blockDim.x) {
+    bool hit = false;
+    uint32_t a = 0, b = 0;
+    if (t < total) hit = config_pair(bb, links, tpl, n_tpl, g0, t, &a, &b);
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if (!m) continue;
+    unsigned base = 0;
+    if (lane == (unsigned)(__ffs(m) - 1)) base = atomicAdd(n_pairs, (unsigned)__popc(m));
+    base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
+    const unsigned pos = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+    if (hit && pos < capacity) {
+      first[pos] = a;
+      second[pos] = b;
+      entry[pos] = (uint32_t)(t % n_tpl);
+    }
+  }
+}
+
 // ---- hfb_env_distance's rounds (BpDistState in hfb_broadphase.h) -------------------------------------------------
 // order-preserving key of a double: keys compare as the values do, -0 and +0 share one key (NaN is never keyed)
 __device__ __forceinline__ unsigned long long dist_key(double d) {
@@ -699,6 +725,94 @@ __global__ void __launch_bounds__(256) k_cfg_take(BpDistState st, CfgItems it, B
   }
 }
 
+// ---- hfb_env_collide_motions (BpMotions in hfb_broadphase.h) -------------------------------------------------------
+// no witness: first_invalid -1, kind -1, first = second = UINT32_MAX, CollisionResult::clear()'s record
+// (collision_data.h:483-489)
+__global__ void __launch_bounds__(256) k_mot_init(unsigned n, BpMotions ms) {
+  const unsigned m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n) return;
+  if (ms.sample) {
+    ms.sample[m] = 0xffffffffu;
+    ms.ord[m] = ~0ull;
+  }
+  if (ms.first_invalid) ms.first_invalid[m] = -1;
+  if (ms.kind) ms.kind[m] = -1;
+  if (ms.first) ms.first[m] = 0xffffffffu;
+  if (ms.second) ms.second[m] = 0xffffffffu;
+  if (ms.rec) {
+    hfb_contact r;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    r.distance = nan;
+    for (int k = 0; k < 3; ++k) r.p1[k] = r.p2[k] = r.normal[k] = r.pos[k] = nan;
+    r.distance_lower_bound = DBL_MAX;
+    r.b1 = r.b2 = -1;
+    r.status = r.num_contacts = r.iterations = r._pad = 0;
+    ms.rec[m] = r;
+  }
+}
+// the colliding candidates of one reduction; the motion of configuration g is the last motion of the range that starts
+// at or before it (an empty motion starts where the next one does)
+struct MotItems {
+  const hfb_contact* r;
+  const uint32_t *pf, *ps, *pk;
+  unsigned n, split, links, n_b, second_base;
+};
+__device__ __forceinline__ bool mot_item(const BpMotions& ms, const MotItems& it, unsigned p, unsigned* m, unsigned* k) {
+  if (p >= it.n || it.r[p].num_contacts == 0) return false;
+  const unsigned g = it.pf[p] / it.links;
+  unsigned lo = ms.m0, hi = ms.m1;  // off[lo] <= g < off[hi]
+  while (hi - lo > 1) {
+    const unsigned mid = lo + (hi - lo) / 2;
+    if (ms.off[mid] <= g) lo = mid;
+    else hi = mid;
+  }
+  *m = lo;
+  *k = g - ms.off[lo];
+  return true;
+}
+__device__ __forceinline__ unsigned long long mot_ord(const MotItems& it, unsigned p) {
+  if (p < it.split) {
+    const unsigned i = it.pf[p] % it.links;
+    return (unsigned long long)i * it.n_b + (it.ps[p] - it.second_base);
+  }
+  return (unsigned long long)it.links * it.n_b + it.pk[p];
+}
+// three passes as k_cfg_min / k_cfg_argmin / k_cfg_take: the smallest colliding sample per motion (and the colliding
+// candidates of each kind counted), the lowest ordinal at that sample, then the gather of the winner
+__global__ void __launch_bounds__(256) k_mot_min(BpMotions ms, MotItems it, unsigned* n_colliding) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned m, k;
+  const bool hit = mot_item(ms, it, p, &m, &k);
+  if (hit) atomicMin(ms.sample + m, k);
+  const unsigned me = __ballot_sync(0xffffffffu, hit && p < it.split), mself = __ballot_sync(0xffffffffu, hit && p >= it.split);
+  if ((threadIdx.x & 31u) == 0) {
+    if (me) atomicAdd(n_colliding, (unsigned)__popc(me));
+    if (mself) atomicAdd(n_colliding + 1, (unsigned)__popc(mself));
+  }
+}
+__global__ void __launch_bounds__(256) k_mot_argmin(BpMotions ms, MotItems it) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned m, k;
+  if (mot_item(ms, it, p, &m, &k) && k == ms.sample[m]) atomicMin(ms.ord + m, mot_ord(it, p));
+}
+__global__ void __launch_bounds__(256) k_mot_take(BpMotions ms, MotItems it) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned m, k;
+  if (!mot_item(ms, it, p, &m, &k) || k != ms.sample[m] || mot_ord(it, p) != ms.ord[m]) return;
+  // (ordinals are unique within a configuration: one candidate per motion gets here)
+  const bool env = p < it.split;
+  if (ms.kind) ms.kind[m] = env ? 0 : 1;
+  if (ms.first) ms.first[m] = it.pf[p];
+  if (ms.second) ms.second[m] = env ? it.ps[p] - it.second_base : it.ps[p];
+  if (ms.rec) ms.rec[m] = it.r[p];
+}
+__global__ void __launch_bounds__(256) k_mot_final(BpMotions ms) {
+  const unsigned m = ms.m0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= ms.m1) return;
+  const unsigned k = ms.sample[m];
+  ms.first_invalid[m] = k == 0xffffffffu ? -1 : (int32_t)k;
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -914,12 +1028,20 @@ int bp_cross_pairs_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size
 
 int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
                            size_t num_configs, uint32_t* d_first, uint32_t* d_second, size_t capacity, unsigned* d_n_pairs,
-                           int num_sms, cudaStream_t s, int* launches) {
+                           int num_sms, cudaStream_t s, int* launches, uint32_t* d_entry) {
   const size_t total = num_configs * n_tpl;
   if (total == 0) return 0;
   if (num_sms < 1) num_sms = 1;
   size_t nb = (total + 127) / 128;
   if (nb > (size_t)num_sms * 16u) nb = (size_t)num_sms * 16u;
+  if (d_entry) {
+    k_config_entry_pairs<<<(unsigned)nb, 128, 0, s>>>(d_aabbs, (unsigned)links, d_tpl, (unsigned)n_tpl, (unsigned)g0, total,
+                                                      d_first, d_second, d_entry,
+                                                      (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity),
+                                                      d_n_pairs);
+    *launches += 1;
+    return (int)cudaGetLastError();
+  }
   k_config_pairs<<<(unsigned)nb, 128, 0, s>>>(d_aabbs, (unsigned)links, d_tpl, (unsigned)n_tpl, (unsigned)g0, total, d_first,
                                               d_second, (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity),
                                               d_n_pairs);
@@ -1058,6 +1180,57 @@ int bp_config_dist_reduce_launch(const BpDistState& st, size_t a_lo, size_t a_hi
   k_cfg_argmin<<<nb, 256, 0, s>>>(st, it, cs);
   k_cfg_take<<<nb, 256, 0, s>>>(st, it, cs);
   *launches += 3;
+  return (int)cudaGetLastError();
+}
+
+size_t bp_motions_bytes(size_t n, bool staged) {
+  return up256(n * 4) + up256(n * 8) + (staged ? 3 * up256(n * 4) + up256(n) + n * sizeof(hfb_contact) : 0);
+}
+
+BpMotions bp_motions_carve(void* p, size_t n, bool staged) {
+  unsigned char* c = static_cast<unsigned char*>(p);
+  BpMotions ms{};
+  ms.sample = reinterpret_cast<unsigned*>(c); c += up256(n * 4);
+  ms.ord = reinterpret_cast<unsigned long long*>(c); c += up256(n * 8);
+  if (!staged) return ms;
+  ms.first_invalid = reinterpret_cast<int32_t*>(c); c += up256(n * 4);
+  ms.first = reinterpret_cast<uint32_t*>(c); c += up256(n * 4);
+  ms.second = reinterpret_cast<uint32_t*>(c); c += up256(n * 4);
+  ms.kind = reinterpret_cast<int8_t*>(c); c += up256(n);
+  ms.rec = reinterpret_cast<hfb_contact*>(c);
+  return ms;
+}
+
+int bp_motions_init_launch(size_t n, const BpMotions& ms, cudaStream_t s, int* launches) {
+  if (n == 0) return 0;
+  k_mot_init<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((unsigned)n, ms);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_motions_reduce_launch(const hfb_contact* d_recs, const uint32_t* d_first, const uint32_t* d_second,
+                             const uint32_t* d_entry, size_t n, size_t split, size_t links, size_t n_b,
+                             uint32_t second_base, bool witness, const BpMotions& ms, unsigned* d_n_colliding,
+                             cudaStream_t s, int* launches) {
+  if (n == 0) return 0;
+  const MotItems it{d_recs, d_first, d_second, d_entry, (unsigned)n, (unsigned)split, (unsigned)links, (unsigned)n_b,
+                    second_base};
+  const unsigned nb = (unsigned)((n + 255) / 256);
+  k_mot_min<<<nb, 256, 0, s>>>(ms, it, d_n_colliding);
+  *launches += 1;
+  if (witness) {
+    k_mot_argmin<<<nb, 256, 0, s>>>(ms, it);
+    k_mot_take<<<nb, 256, 0, s>>>(ms, it);
+    *launches += 2;
+  }
+  return (int)cudaGetLastError();
+}
+
+int bp_motions_final_launch(const BpMotions& ms, cudaStream_t s, int* launches) {
+  const unsigned n = ms.m1 - ms.m0;
+  if (n == 0 || !ms.first_invalid) return 0;
+  k_mot_final<<<(n + 255) / 256, 256, 0, s>>>(ms);
+  *launches += 1;
   return (int)cudaGetLastError();
 }
 

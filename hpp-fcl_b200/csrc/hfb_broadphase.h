@@ -51,10 +51,10 @@ int bp_cross_query_launch(size_t n_a, const double* d_aabbs_a, size_t a_lo, size
 // the self pairs of configurations [g0, g0 + num_configs) of L = `links` objects each (config_pair of
 // hfb_broadphase.cuh; d_tpl: n_tpl pairs of link indices, validated) -> (d_first, d_second), APPENDED after the pairs
 // *d_n_pairs already counts; at most `capacity` stored in all.  Returns a cudaError_t as int; *launches += kernels
-// launched.
+// launched.  d_entry (may be null): each pair's template entry, stored at its position in the list.
 int bp_config_pairs_launch(const double* d_aabbs, size_t links, const uint32_t* d_tpl, size_t n_tpl, size_t g0,
                            size_t num_configs, uint32_t* d_first, uint32_t* d_second, size_t capacity, unsigned* d_n_pairs,
-                           int num_sms, cudaStream_t s, int* launches);
+                           int num_sms, cudaStream_t s, int* launches, uint32_t* d_entry = nullptr);
 // ---- hfb_env_distance: each A object's nearest B object, found in rounds of growing radius (DESIGN.md §3) ----------
 // Round k runs distance() on the pairs whose B box overlaps the A box inflated by rho_k = min(cell * 8^k, max_distance)
 // (outward rounding) and did not overlap the round before's; an A object is settled once its best eligible distance is
@@ -123,6 +123,36 @@ int bp_config_dist_reduce_launch(const BpDistState& st, size_t a_lo, size_t a_hi
                                  const hfb_distance_result* d_recs, const uint32_t* d_first, const uint32_t* d_second,
                                  const uint32_t* d_entry, size_t n_self, double max_distance, const BpConfigDist& cs,
                                  unsigned* d_n_unsupported, cudaStream_t s, int* launches);
+// ---- hfb_env_collide_motions: each motion's first colliding sample and its first colliding pair (DESIGN.md §3) ----
+// Over the collide() records of hfb_env_collide_configs' candidate list (environment pairs before `split`, self pairs
+// from there on), three passes touch the colliding ones: the smallest sample per motion, then the lowest pair ordinal
+// at that sample (environment: link * n_b + index in B; self: L * n_b + template entry), then the gather of the
+// winner.  Per-motion state, n_motions each (bp_motions_bytes(n_motions) bytes of the caller's; `staged` adds room for
+// the outputs, which the host form downloads from there):
+struct BpMotions {
+  const uint32_t* off;          // the motion offsets, n_motions + 1 (device copy)
+  unsigned m0, m1;              // the motions checked
+  unsigned* sample;             // the smallest colliding sample; UINT32_MAX: none
+  unsigned long long* ord;      // the lowest ordinal among the colliding pairs at `sample`
+  int32_t* first_invalid;       // outputs, each may be null
+  int8_t* kind;
+  uint32_t* first;
+  uint32_t* second;
+  hfb_contact* rec;
+};
+size_t bp_motions_bytes(size_t n_motions, bool staged);
+BpMotions bp_motions_carve(void* p, size_t n_motions, bool staged);
+// every motion without a witness: the state (when ms.sample is set) and the outputs that are set
+int bp_motions_init_launch(size_t n_motions, const BpMotions& ms, cudaStream_t s, int* launches);
+// the n records d_recs of the candidates (d_first, d_second, d_entry: the self pairs' template entries) into the
+// per-motion state and, when `witness`, the outputs kind, first, second and rec (second_base taken off the environment
+// pairs' second index); the colliding candidates before / from `split` on are added to d_n_colliding[0] / [1]
+int bp_motions_reduce_launch(const hfb_contact* d_recs, const uint32_t* d_first, const uint32_t* d_second,
+                             const uint32_t* d_entry, size_t n, size_t split, size_t links, size_t n_b,
+                             uint32_t second_base, bool witness, const BpMotions& ms, unsigned* d_n_colliding,
+                             cudaStream_t s, int* launches);
+// first_invalid of the motions checked from the state (-1: none)
+int bp_motions_final_launch(const BpMotions& ms, cudaStream_t s, int* launches);
 // hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
                          const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,

@@ -929,6 +929,7 @@ struct hfb_ctx {
   DevBuf sc_tpl;                                                   // hfb_env_collide_configs: the self-pair template
   DevBuf sc_dist, sc_drec;  // hfb_env_distance: the per-A state (hfb::BpDistState), a round's distance() records
   DevBuf sc_cdist;          // hfb_env_distance_configs: the per-configuration state (hfb::BpConfigDist)
+  DevBuf sc_moff, sc_mot;   // hfb_env_collide_motions: the motion offsets, the per-motion state (hfb::BpMotions)
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   uint64_t commits = 0, clears = 0;
@@ -2554,11 +2555,12 @@ static int find_all(hfb_ctx* ctx, cudaStream_t s, std::initializer_list<DevBuf*>
 // (d_h, d_tf: n objects): the boxes of its first n_boxes objects, the candidates (find_pairs(d_bb, pf, ps, capacity,
 // d_count, &launches) launches a pair finder, all pairs counted in *d_count, at most `capacity` stored) and collide() of
 // every candidate over the table, into ctx->sc_out (none when there are no candidates or under minus_inf).
-// split_out (may be null): the counter's second word, which a finder may set, read with the count.
+// split_out (may be null): the counter's second word, which a finder may set, read with the count.  entry (may be
+// null): a third candidate list the finder fills, grown with the other two.
 template <class FindPairs>
 static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32_t* d_h, const hfb_transform* d_tf,
                             size_t n_boxes, FindPairs find_pairs, const hfb_collision_request* req, bool minus_inf,
-                            unsigned* cand_out, unsigned* split_out = nullptr) {
+                            unsigned* cand_out, unsigned* split_out = nullptr, DevBuf* entry = nullptr) {
   CK(ctx->sc_bb.reserve(n_boxes * 48));
   CK(ctx->sc_cnt.reserve(16));
   double* d_bb = static_cast<double*>(ctx->sc_bb.p);
@@ -2570,7 +2572,10 @@ static int scene_candidates(hfb_ctx* ctx, cudaStream_t s, size_t n, const uint32
   auto find = [&](size_t cap, int* nl) {
     return find_pairs(d_bb, static_cast<uint32_t*>(ctx->sc_pf.p), static_cast<uint32_t*>(ctx->sc_ps.p), cap, d_cnt, nl);
   };
-  if (int rc = find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps}, d_cnt, find, words, split_out ? 2 : 1)) return rc;
+  const int n_words = split_out ? 2 : 1;
+  if (int rc = entry ? find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps, entry}, d_cnt, find, words, n_words)
+                     : find_all(ctx, s, {&ctx->sc_pf, &ctx->sc_ps}, d_cnt, find, words, n_words))
+    return rc;
   const unsigned cand = words[0];
   if (split_out) *split_out = words[1];
   *cand_out = cand;
@@ -3051,9 +3056,41 @@ static int configs_output(hfb_ctx* ctx, unsigned cand, unsigned split, uint32_t 
   return HFB_OK;
 }
 
-// hfb_env_collide_configs (the template in ctx->sc_tpl): one candidate list -- the environment pairs against the
-// built grid, then, after the split is noted in the counter's second word, the self pairs appended to it -- one narrow
-// phase over the table [A; B], then the outputs
+// The candidates of a configurations query (the template in ctx->sc_tpl) and their collide() records in ctx->sc_out:
+// one candidate list -- the environment pairs against the built grid, then, after the split is noted in the counter's
+// second word, the self pairs appended to it -- and one narrow phase over the table [A; B].  entries: each self pair's
+// template entry in ctx->sc_f, at its position in the list.
+static int configs_candidates(hfb_ctx* ctx, hfb_env* e, size_t n_a, const ConfigTpl& t, const hfb_collision_request* req,
+                              bool minus_inf, bool entries, cudaStream_t s, unsigned* cand, unsigned* split) {
+  const size_t n_b = e->n_b, links = t.links, n_tpl = t.n, g0 = t.g0, ng = t.ng;
+  const size_t a_lo = g0 * links, a_hi = (g0 + ng) * links;
+  const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
+  const double* bb_b = static_cast<const double*>(e->bb.p);
+  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+  CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
+  auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+    int rc = 0;
+    if (n_b) {
+      rc = bp_cross_query_reset(g, d_cnt, s);
+      if (!rc)
+        rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
+                                   ctx->bp_scratch.p, ctx->num_sms, s, nl);
+    } else {
+      rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
+    }
+    if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
+    if (!rc)
+      rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl,
+                                  entries ? static_cast<uint32_t*>(ctx->sc_f.p) : nullptr);
+    return rc;
+  };
+  const size_t off = e->head - n_a;
+  return scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
+                          static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, cand, split,
+                          entries ? &ctx->sc_f : nullptr);
+}
+
+// hfb_env_collide_configs: the candidates and their records (configs_candidates), then the outputs
 struct EnvCollideConfigs {
   const hfb_collision_request* req;
   const hfb_configs_out* out;
@@ -3072,33 +3109,9 @@ struct EnvCollideConfigs {
   }
   bool empty(const hfb_env* e, size_t n_a) const { return n_a == 0 || t.ng == 0 || (e->n_b == 0 && t.n == 0); }
   int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
-    const cudaStream_t s = o.s;
-    const size_t n_b = e->n_b, links = t.links, n_tpl = t.n, g0 = t.g0, ng = t.ng;
-    const size_t a_lo = g0 * links, a_hi = (g0 + ng) * links;
-    const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
-    const double* bb_b = static_cast<const double*>(e->bb.p);
-    const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
-    CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
-    auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
-      int rc = 0;
-      if (n_b) {
-        rc = bp_cross_query_reset(g, d_cnt, s);
-        if (!rc)
-          rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
-                                     ctx->bp_scratch.p, ctx->num_sms, s, nl);
-      } else {
-        rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
-      }
-      if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
-      if (!rc) rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
-      return rc;
-    };
-    const size_t off = e->head - n_a;
+    const size_t links = t.links;
     unsigned cand = 0, split = 0;
-    if (int rc = scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
-                                  static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, &cand,
-                                  &split))
-      return rc;
+    if (int rc = configs_candidates(ctx, e, n_a, t, req, minus_inf, false, o.s, &cand, &split)) return rc;
     CK(o.count(out->env.n_candidates, split));
     CK(o.count(out->self.n_candidates, cand - split));
     if (cand == 0 || minus_inf) {
@@ -3322,6 +3335,147 @@ struct EnvDistanceConfigs {
   }
 };
 
+// hfb_env_collide_motions' outputs, checked before the context is looked at
+static bool motions_ok(const hfb_motions_out* o) { return o && (o->first_invalid || o->kind || o->contacts); }
+
+// the record of a motion without a witness: CollisionResult::clear() (collision_data.h:483-489), as k_mot_init writes it
+static hfb_contact cleared_contact() {
+  hfb_contact r;
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  r.distance = nan;
+  for (int k = 0; k < 3; ++k) r.p1[k] = r.p2[k] = r.normal[k] = r.pos[k] = nan;
+  r.distance_lower_bound = DBL_MAX;
+  r.b1 = r.b2 = -1;
+  r.status = r.num_contacts = r.iterations = r._pad = 0;
+  return r;
+}
+
+// hfb_env_collide_motions (the template in ctx->sc_tpl, the offsets uploaded into ctx->sc_moff): the candidates and
+// records of hfb_env_collide_configs over the range's configurations (configs_candidates, with the self pairs' template
+// entries when a witness is wanted), then per motion the first colliding sample and its first colliding pair
+// (hfb::BpMotions, in ctx->sc_mot).  t.g0 and t.ng are set by motions_args.
+struct EnvCollideMotions {
+  const hfb_collision_request* req;
+  const hfb_motions_out* out;
+  ConfigTpl t;
+  size_t n_motions;
+  const uint32_t* offsets;
+  size_t first_motion, num_motions;
+  bool minus_inf = false;
+
+  const ConfigTpl* tpl() const { return &t; }
+  bool witness() const { return out->kind || out->first || out->second || out->contacts; }
+  int check(hfb_ctx* ctx) { return collide_prelude(ctx, req, &minus_inf); }
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t) const {
+    for (uint32_t* c : {out->n_env_candidates, out->n_env_colliding, out->n_self_candidates, out->n_self_colliding})
+      CK(o.zero(c, sizeof(uint32_t)));
+    const size_t n = n_motions;
+    if (o.dev) {  // (on the caller's stream)
+      BpMotions ms{};
+      ms.first_invalid = out->first_invalid;
+      ms.kind = out->kind;
+      ms.first = out->first;
+      ms.second = out->second;
+      ms.rec = out->contacts;
+      int nl = 0;
+      if (bp_motions_init_launch(n, ms, o.s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_mot_init launch failed");
+      ctx->stats.kernel_launches += (uint64_t)nl;
+      return HFB_OK;
+    }
+    if (out->first_invalid) std::fill(out->first_invalid, out->first_invalid + n, -1);
+    if (out->kind) std::fill(out->kind, out->kind + n, (int8_t)-1);
+    if (out->first) std::fill(out->first, out->first + n, 0xffffffffu);
+    if (out->second) std::fill(out->second, out->second + n, 0xffffffffu);
+    if (out->contacts) std::fill(out->contacts, out->contacts + n, cleared_contact());
+    return HFB_OK;
+  }
+  bool empty(const hfb_env* e, size_t n_a) const { return n_a == 0 || t.ng == 0 || (e->n_b == 0 && t.n == 0); }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const bool wit = witness();
+    unsigned cand = 0, split = 0;
+    if (int rc = configs_candidates(ctx, e, n_a, t, req, minus_inf, wit, s, &cand, &split)) return rc;
+    CK(o.count(out->n_env_candidates, split));
+    CK(o.count(out->n_self_candidates, cand - split));
+    if (cand == 0 || minus_inf) {  // (no colliding pair: the zeroed counts and the no-witness outputs stand)
+      CK(o.finish());
+      return HFB_OK;
+    }
+    const size_t n = n_motions;
+    CK(ctx->sc_moff.reserve((n + 1) * 4));
+    CK(cudaMemcpyAsync(ctx->sc_moff.p, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, s));
+    CK(ctx->sc_mot.reserve(bp_motions_bytes(n, !o.dev)));
+    BpMotions ms = bp_motions_carve(ctx->sc_mot.p, n, !o.dev);  // (the host form stages its outputs there)
+    ms.off = static_cast<const uint32_t*>(ctx->sc_moff.p);
+    ms.m0 = (unsigned)first_motion;
+    ms.m1 = (unsigned)(first_motion + num_motions);
+    if (o.dev) {
+      ms.first_invalid = out->first_invalid;
+      ms.kind = out->kind;
+      ms.first = out->first;
+      ms.second = out->second;
+      ms.rec = out->contacts;
+    } else {
+      if (!out->first_invalid) ms.first_invalid = nullptr;
+      if (!out->kind) ms.kind = nullptr;
+      if (!out->first) ms.first = nullptr;
+      if (!out->second) ms.second = nullptr;
+      if (!out->contacts) ms.rec = nullptr;
+    }
+    BpMotions state = ms;  // the device form's outputs hold zero()'s no-witness values already
+    if (o.dev) state.first_invalid = nullptr, state.kind = nullptr, state.first = state.second = nullptr, state.rec = nullptr;
+    unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+    CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
+    int nl = 0;
+    if (bp_motions_init_launch(n, state, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_mot_init launch failed");
+    if (bp_motions_reduce_launch(static_cast<const hfb_contact*>(ctx->sc_out.p), static_cast<const uint32_t*>(ctx->sc_pf.p),
+                                 static_cast<const uint32_t*>(ctx->sc_ps.p), static_cast<const uint32_t*>(ctx->sc_f.p), cand,
+                                 split, t.links, e->n_b, (uint32_t)n_a, wit, ms, d_cnt + 1, s, &nl) != 0)
+      return fail(ctx, HFB_ERR_CUDA, "k_mot_min launch failed");
+    if (bp_motions_final_launch(ms, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_mot_final launch failed");
+    ctx->stats.kernel_launches += (uint64_t)nl;
+    if (!o.dev) {
+      CK(o.copy(out->first_invalid, ms.first_invalid, n * 4));
+      CK(o.copy(out->kind, ms.kind, n));
+      CK(o.copy(out->first, ms.first, n * 4));
+      CK(o.copy(out->second, ms.second, n * 4));
+      CK(o.copy(out->contacts, ms.rec, n * sizeof(hfb_contact)));
+    }
+    CK(o.copy(out->n_env_colliding, d_cnt + 1, sizeof(unsigned)));
+    CK(o.copy(out->n_self_colliding, d_cnt + 2, sizeof(unsigned)));
+    CK(o.finish());
+    return HFB_OK;
+  }
+};
+
+// hfb_env_collide_motions' arguments beyond the pointers: the offsets, the motion range, then configs_args over the
+// range's configurations (into q.t)
+static int motions_args(hfb_ctx* ctx, size_t n_a, EnvCollideMotions& q) {
+  const size_t links = q.t.links, n = q.n_motions;
+  const uint32_t* off = q.offsets;
+  if (links == 0 || n_a % links) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "n_a is not a multiple of links_per_config");
+  if (n > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "too many motions");
+  if (off[0] != 0) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "motion offsets do not start at 0");
+  for (size_t m = 0; m < n; ++m) {
+    if (off[m + 1] < off[m]) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "motion offsets decrease");
+    if (off[m + 1] - off[m] > 0x7fffffffu) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "a motion has more than INT32_MAX samples");
+  }
+  if (off[n] != n_a / links) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "motion offsets do not end at n_configs");
+  if (q.first_motion > n || q.num_motions > n - q.first_motion)
+    return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "motion range past the end");
+  q.t.g0 = off[q.first_motion];
+  q.t.ng = off[q.first_motion + q.num_motions] - q.t.g0;
+  return configs_args(ctx, n_a, links, q.t.n, q.t.pairs, q.t.g0, q.t.ng);
+}
+
+// a query's arguments beyond the pointers: those of a configurations query, or of a motions query
+template <class Query>
+static int query_args(hfb_ctx* ctx, size_t n_a, Query& q) {
+  const ConfigTpl* t = q.tpl();
+  return t ? configs_args(ctx, n_a, t->links, t->n, t->pairs, t->g0, t->ng) : HFB_OK;
+}
+static int query_args(hfb_ctx* ctx, size_t n_a, EnvCollideMotions& q) { return motions_args(ctx, n_a, q); }
+
 // The frame of the hfb_env_* queries (EnvCollide, EnvCollideConfigs, EnvDistance, EnvDistanceConfigs), with their
 // pointers checked: the lock, the query's and the env's checks, A uploaded into the env's table in front of B (and
 // the template `tpl` of a configurations query into ctx->sc_tpl), then the query.  Host form (Form::host): A and the
@@ -3338,8 +3492,7 @@ static int env_call(hfb_ctx* ctx, hfb_env* env, Form form, void* stream, size_t 
   if (int rc = q.check(ctx)) return rc;
   if (int rc = env_ready(ctx, env)) return rc;
   if (n_a > 0xffffffffull || n_a + env->n_b > 0xffffffffull) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "scene too large");
-  if (tpl)
-    if (int rc = configs_args(ctx, n_a, tpl->links, tpl->n, tpl->pairs, tpl->g0, tpl->ng)) return rc;
+  if (int rc = query_args(ctx, n_a, q)) return rc;
   QueryOut o{dev ? static_cast<cudaStream_t>(stream) : ctx->slots[0].stream, dev};
   if (!dev) {
     if (int rc = check_handles(ctx, h_a, n_a)) return rc;
@@ -3481,6 +3634,35 @@ int hfb_env_collide_configs_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
   if (!contacts_ok(d_out->env) || !contacts_ok(d_out->self)) return HFB_ERR_INVALID_ARGUMENT;
   return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
                   EnvCollideConfigs{req, d_out, {links_per_config, n_self_pairs, self_pairs, first_config, num_configs}});
+}
+
+// A planner's motion validation (hfb_motions_out in include/hppfcl_b200.h): per motion, a run of configurations, the
+// first sample whose hfb_env_collide_configs verdict would be 1 and the first colliding pair there -- OMPL's
+// DiscreteMotionValidator::checkMotion(s1, s2, lastValid) and hpp-core's discretized path validation over the caller's
+// samples.
+int hfb_env_collide_motions(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                            const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                            const hfb_collision_request* req, const hfb_motions_out* out) {
+  if (!ctx || !env || !req || !motions_ok(out) || !motion_offsets || (n_a && (!handles_a || !tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a,
+                  EnvCollideMotions{req, out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
+                                    motion_offsets, first_motion, num_motions});
+}
+
+int hfb_env_collide_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                   const uint32_t* self_pairs, size_t n_motions, const uint32_t* motion_offsets,
+                                   size_t first_motion, size_t num_motions, const hfb_collision_request* req,
+                                   const hfb_motions_out* d_out, void* stream) {
+  if (!ctx || !env || !req || !motions_ok(d_out) || !motion_offsets || (n_a && (!d_handles_a || !d_tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
+                  EnvCollideMotions{req, d_out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
+                                    motion_offsets, first_motion, num_motions});
 }
 
 // Each A object's nearest B object (hfb_env_distance_out in include/hppfcl_b200.h): the result of

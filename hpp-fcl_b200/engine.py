@@ -78,6 +78,8 @@ def load_library(path=None):
     L.hfb_broadphase_config_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, vp, vp, sz, vp]
     L.hfb_env_distance_configs.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, C.c_double, vp]
     L.hfb_env_distance_configs_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, sz, vp, C.c_double, vp, vp]
+    L.hfb_env_collide_motions.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp]
+    L.hfb_env_collide_motions_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, vp]
     L.hfb_broadphase_config_distance_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, C.c_double, vp, vp, sz, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
@@ -206,6 +208,16 @@ def broadphase_config_distance_pairs(aabbs, links_per_config, self_pairs, max_di
         raise EngineError("hfb_broadphase_config_distance_pairs: %s" % _ERR.get(rc, rc))
     k = min(cnt.value, cap)
     return first[:k], second[:k]
+
+
+def _offsets(offsets):
+    """motion offsets as the C ABI takes them: n_motions + 1 uint32, contiguous"""
+    off = np.asarray(offsets).reshape(-1)
+    if off.shape[0] == 0:
+        raise ValueError("motion offsets: n_motions + 1 values, at least one")
+    if off.dtype.kind not in "ui" or (off.dtype.kind == "i" and (off < 0).any()) or (off > 0xFFFFFFFF).any():
+        raise ValueError("motion offsets: integers in [0, 2^32)")
+    return np.ascontiguousarray(off, dtype=np.uint32)
 
 
 def _ptr(a):
@@ -605,6 +617,50 @@ class Engine:
                                                            tpl.shape[0], _ptr(tpl), first_config,
                                                            n_configs - first_config if num_configs is None else num_configs,
                                                            C.byref(req), float(max_distance), C.byref(out), _ptr(stream)))
+
+    def env_collide_motions(self, env, handles_a, tfs_a, links_per_config, self_pairs, offsets, req=None, first_motion=0,
+                            num_motions=None, witness=True):
+        """motions of configurations (A: configurations of links_per_config objects each, configuration-major, motion m
+        is configurations [offsets[m], offsets[m+1])) against the env and against themselves (hfb_env_collide_motions)
+        -> (first_invalid: per motion the first colliding sample, -1 for none; kind: 0 environment, 1 self, -1 none;
+        first: index in A; second: index in B for kind 0, in A for kind 1, UINT32_MAX for none; contacts: the witness's
+        record; counts = (n_env_candidates, n_env_colliding, n_self_candidates, n_self_colliding)).  witness=False:
+        first_invalid alone, kind, first, second and contacts None"""
+        req = req or P.CollisionRequestPOD()
+        ha, ta = self._objects(handles_a, tfs_a)
+        tpl = _template(self_pairs)
+        off = _offsets(offsets)
+        na, n_motions = ha.shape[0], off.shape[0] - 1
+        first_invalid = np.empty(n_motions, dtype=np.int32)
+        kind = np.empty(n_motions, dtype=np.int8) if witness else None
+        first = np.empty(n_motions, dtype=np.uint32) if witness else None
+        second = np.empty(n_motions, dtype=np.uint32) if witness else None
+        contacts = np.empty(n_motions, dtype=P.contact_dtype) if witness else None
+        nc = np.zeros(4, dtype=np.uint32)
+        out = P.MotionsOut(first_invalid.ctypes.data, *[None if a is None else a.ctypes.data for a in (kind, first, second, contacts)],
+                           *[nc[k:].ctypes.data for k in range(4)])
+        self._check(self.L.hfb_env_collide_motions(self.h, env, na, _ptr(ha), _ptr(ta), int(links_per_config), tpl.shape[0],
+                                                   _ptr(tpl), n_motions, _ptr(off), first_motion,
+                                                   n_motions - first_motion if num_motions is None else num_motions,
+                                                   C.byref(req), C.byref(out)))
+        return first_invalid, kind, first, second, contacts, tuple(int(c) for c in nc)
+
+    def env_collide_motions_device(self, env, n_a, d_handles_a, d_tfs_a, links_per_config, self_pairs, offsets,
+                                   d_first_invalid, d_kind, d_first, d_second, d_contacts, d_counts=(None,) * 4, req=None,
+                                   stream=0, first_motion=0, num_motions=None):
+        """hfb_env_collide_motions_device: A's handles and poses and every output are device pointers, ordered on
+        `stream`; d_counts = (d_n_env_candidates, d_n_env_colliding, d_n_self_candidates, d_n_self_colliding); the
+        template and the offsets are host arrays"""
+        req = req or P.CollisionRequestPOD()
+        tpl = _template(self_pairs)
+        off = _offsets(offsets)
+        n_motions = off.shape[0] - 1
+        out = P.MotionsOut(d_first_invalid, d_kind, d_first, d_second, d_contacts, *d_counts)
+        self._check(self.L.hfb_env_collide_motions_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a),
+                                                          int(links_per_config), tpl.shape[0], _ptr(tpl), n_motions,
+                                                          _ptr(off), first_motion,
+                                                          n_motions - first_motion if num_motions is None else num_motions,
+                                                          C.byref(req), C.byref(out), _ptr(stream)))
 
     @staticmethod
     def _objects(handles, tfs):

@@ -1071,8 +1071,63 @@ class ResidentEnvironment {
                      {nullptr, nullptr, nullptr, d.data(), nullptr, nullptr, nullptr, nullptr});
     return d;
   }
+  /// A planner's motion validation: the robot manager holds configurations laid out as in collide_configurations, the
+  /// samples of each motion one after another in walking order; motion m is configurations [offsets[m], offsets[m+1]).
+  /// Per motion: first_invalid[m], the first sample that collides with the environment or with itself (-1 when none
+  /// does); kind[m]: 0 environment pair, 1 self pair, -1 none; first[m]: index in the robot manager; second[m]: index
+  /// in the environment (kind 0) or in the robot manager (kind 1), UINT32_MAX when none; returns the pairs' contact
+  /// records.  The pair is the first colliding one of that sample: environment pairs by link, then by environment
+  /// index, then self pairs in template order (hfb_env_collide_motions).  Malformed offsets (not starting at 0,
+  /// decreasing, not ending at the number of configurations) or a malformed template throw std::invalid_argument.
+  std::vector<hfb_contact> collide_motions(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                           const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                           const std::vector<uint32_t>& offsets, const CollisionRequest& request,
+                                           std::vector<int32_t>& first_invalid, std::vector<int8_t>& kind,
+                                           std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
+    if (offsets.empty()) throw std::invalid_argument("motion offsets: n_motions + 1 values, at least one");
+    const size_t n = offsets.size() - 1;
+    std::vector<hfb_contact> rec(n);
+    first_invalid.resize(n);
+    kind.resize(n);
+    first.resize(n);
+    second.resize(n);
+    check_motions(robot, links_per_config, self_pairs, offsets, request,
+                  {first_invalid.data(), kind.data(), first.data(), second.data(), rec.data(), nullptr, nullptr, nullptr,
+                   nullptr});
+    return rec;
+  }
+  /// the first colliding samples alone (no pair records come back)
+  std::vector<int32_t> first_invalid_samples(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                             const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                             const std::vector<uint32_t>& offsets,
+                                             const CollisionRequest& request = CollisionRequest()) {
+    if (offsets.empty()) throw std::invalid_argument("motion offsets: n_motions + 1 values, at least one");
+    std::vector<int32_t> first_invalid(offsets.size() - 1);
+    check_motions(robot, links_per_config, self_pairs, offsets, request,
+                  {first_invalid.data(), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr});
+    return first_invalid;
+  }
 
  private:
+  void check_motions(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                     const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const std::vector<uint32_t>& offsets,
+                     const CollisionRequest& request, const hfb_motions_out& out) {
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    std::vector<uint32_t> tpl;
+    for (const auto& p : self_pairs) {
+      tpl.push_back(p.first);
+      tpl.push_back(p.second);
+    }
+    const size_t n = offsets.size() - 1;
+    // no motions: the callers' vectors are empty and may hand out null data(), which the C ABI would take for
+    // outputs not asked for; one slot stands in (nothing is written to it)
+    int32_t none = -1;
+    hfb_motions_out o = out;
+    if (n == 0) o.first_invalid = &none;
+    C.check(hfb_env_collide_motions(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(), links_per_config,
+                                    self_pairs.size(), tpl.data(), n, offsets.data(), 0, n, &q, &o));
+  }
   void distance_configs(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
                         const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const DistanceRequest& request,
                         FCL_REAL max_distance, const hfb_configs_distance_out& out) {

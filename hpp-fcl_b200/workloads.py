@@ -340,6 +340,55 @@ def robot_vs_environment(n_configs=1024, n_links=16, n_env=100_000, room=None, s
                 n_configs=K, n_links=L)
 
 
+def robot_motions(n_motions, n_links=16, n_env=100_000, room=None, seed=0xFC1 + 7, target_pairs=1_000_000,
+                  joint_range=1.2, max_step=1.0, resolution=0.025):
+    """A planner's motion validation: n_motions straight-line joint-space motions of robot_vs_environment's chain robot,
+    in its room and against its environment.  A motion's joints are the base yaw and the n_links - 1 bending joints
+    (within +-joint_range rad), its base position fixed in the room.  Each motion goes from a random start towards a
+    goal up to 1.25 steps away for at most `max_step` (Euclidean, joint space), as an RRT extension does, and is sampled every
+    `resolution` rad along it, end points included, so sample counts vary.  The samples' poses come from forward
+    kinematics, one configuration per sample, motion after motion.  `room` defaults to robot_vs_environment's for the
+    total sample count.
+    -> robot_vs_environment's dict with tf_a / geom_a holding the samples (n_configs of them), plus `offsets`
+    (n_motions + 1: motion m is configurations [offsets[m], offsets[m+1])), `n_motions` and `q` (the joint values,
+    n_configs x n_links)."""
+    rng = np.random.default_rng(seed)
+    K, L = n_motions, n_links
+    lo = np.concatenate([[-np.pi], np.full(L - 1, -joint_range)])
+    hi = np.concatenate([[np.pi], np.full(L - 1, joint_range)])
+    q0 = lo + (hi - lo) * rng.random((K, L))
+    d = rng.standard_normal((K, L))  # towards a goal up to 1.25 steps away, in a random direction
+    d *= (1.25 * max_step * rng.random(K) / np.maximum(np.linalg.norm(d, axis=1), 1e-300))[:, None]
+    d *= (max_step / np.maximum(np.linalg.norm(d, axis=1), max_step))[:, None]
+    d[:, 1:] = np.clip(q0[:, 1:] + d[:, 1:], lo[1:], hi[1:]) - q0[:, 1:]  # (the bending joints stay in range)
+    n_samples = 1 + np.ceil(np.linalg.norm(d, axis=1) / resolution).astype(np.int64)
+    offsets = np.concatenate([[0], np.cumsum(n_samples)]).astype(np.uint32)
+    total = int(offsets[-1])
+    w = robot_vs_environment(total, n_links, n_env, room, seed=seed, target_pairs=target_pairs, joint_range=joint_range)
+    base = np.repeat(rng.random((K, 3)) * np.array([w["room"], w["room"], 0.0]), n_samples, axis=0)
+    motion = np.repeat(np.arange(K), n_samples)
+    step = np.arange(total) - offsets[motion]
+    frac = step / np.maximum(n_samples[motion] - 1, 1)
+    q = q0[motion] + frac[:, None] * d[motion]
+
+    def fk(base, q):  # the chain of robot_vs_environment: joint k turns about z (k even) or y (k odd)
+        R = np.broadcast_to(np.eye(3), (len(q), 3, 3))
+        p = base.copy()
+        Rs, Ts = np.empty((len(q), L, 3, 3)), np.empty((len(q), L, 3))
+        for k in range(L):
+            R = R @ _axis_rotations(2 if k % 2 == 0 else 1, q[:, k])
+            axis = R[:, :, 2]
+            Rs[:, k] = R
+            Ts[:, k] = p + 0.5 * w["link_len"] * axis
+            p = p + w["link_len"] * axis
+        return P.make_transforms(Rs.reshape(-1, 3, 3), Ts.reshape(-1, 3))
+
+    w["tf_a"] = fk(base, q)
+    w["geom_a"] = np.tile(w["geom_a"][:L], total)
+    w.update(offsets=offsets, n_motions=K, q=q)
+    return w
+
+
 def chain_self_pairs(n_links, skip=2):
     """the self-pair template of a chain: every link pair (i, j) with j >= i + skip (neighbours touch at their joint
     and are not checked, as an SRDF disables adjacent links) -> (P, 2) uint32; 105 pairs for 16 links"""

@@ -626,6 +626,66 @@ int hfb_broadphase_config_distance_pairs(size_t n_a, const double* aabbs, size_t
                                          double max_distance, uint32_t* first, uint32_t* second, size_t capacity,
                                          size_t* n_pairs);
 
+/* ---- a planner's motion validation: each motion's first colliding sample and the pair that collides there ---------
+ * A, the template and the configuration layout are those of hfb_env_collide_configs (object g*L + i is link i of
+ * configuration g), checked the same way.  The library does not interpolate: the caller samples each motion (forward
+ * kinematics is the caller's) and lays its configurations out one after another, in walking order.  There are
+ * n_motions motions; motion_offsets holds n_motions + 1 uint32 values in HOST memory (in both forms, as the template):
+ * motion m is configurations [offsets[m], offsets[m+1]), and sample k of motion m is configuration offsets[m] + k.
+ * offsets[0] != 0, decreasing offsets, offsets[n_motions] != n_configs or a motion of more than INT32_MAX samples is
+ * HFB_ERR_INVALID_ARGUMENT.  An empty motion is allowed and is valid.  Only motions [first_motion, first_motion +
+ * num_motions) are checked (one GPU's share); a range past n_motions is HFB_ERR_INVALID_ARGUMENT.  The configurations
+ * checked are those of the range's motions, with exactly the candidates, collide() calls (o1, o2) and records
+ * hfb_env_collide_configs has over that configuration range: a sample collides iff its verdict there would be 1.
+ * Within a configuration the pairs are ordered as in hfb_env_distance_configs: environment pairs by link, then by B
+ * index; then self pairs in template order.  Per motion m:
+ *   first_invalid[m]: the smallest k whose sample collides, -1 when none does or the motion is empty (int32).  To
+ *                     validate from the end (hpp-core's `reverse`), lay the samples out end first.
+ *   kind[m]:          0 environment pair, 1 self pair, -1 none (int8).
+ *   first[m], second[m]: the witness, the first colliding pair in the order above of sample first_invalid[m]: its index
+ *                     in A, and its index in B (kind 0) or in A (kind 1); both UINT32_MAX without a witness.
+ *   contacts[m]:      the witness's record, byte for byte the one hfb_env_collide_configs returns for that pair;
+ *                     without a witness the cleared CollisionResult (collision_data.h:483-489): distance_lower_bound
+ *                     DBL_MAX, distance, p1, p2, normal and pos quiet NaN, b1 = b2 = -1, status, num_contacts,
+ *                     iterations and _pad 0.
+ *   Motions outside the range get the no-witness values.  first_invalid, kind and contacts may each be null but not
+ *   all three; first and second may be null.  With kind, first, second and contacts all null no witness is sought.
+ *   n_env_candidates, n_env_colliding, n_self_candidates, n_self_colliding (may be null): what hfb_env_collide_configs
+ *   reports for the same configuration range.  Every sample is checked (no early exit past a motion's first colliding
+ *   sample), so the counts do not depend on scheduling.  Counts are 32 bits.
+ * This is OMPL's DiscreteMotionValidator::checkMotion(s1, s2, lastValid) over the caller's samples, and hpp-core's
+ * discretized path validation, whose PathValidationReport carries the colliding pair and its CollisionResult.
+ * An env with no objects still checks the self pairs.  Handles, the env's validity and the request are checked as
+ * hfb_env_collide checks them; security_margin == -inf gives no contacts and every motion valid.  A refused call
+ * writes nothing.
+ *   hfb_env_collide_motions: HOST buffers, blocking.
+ *   hfb_env_collide_motions_device: A's handles and poses and every output in DEVICE memory, ordered on `cuda_stream`
+ *     (the template and the offsets stay in host memory).  It blocks where hfb_env_collide_configs_device does: on
+ *     `cuda_stream` for the candidate count (twice when the candidates outgrow the context's candidate lists, which
+ *     then grow), and growing a context or env buffer (the candidate lists, the records, the per-motion state, the
+ *     env's table when A has more objects than any query before) allocates device memory, which waits for the whole
+ *     device.  Later host calls on the context wait for it. */
+typedef struct hfb_motions_out {
+  int32_t* first_invalid;
+  int8_t* kind;
+  uint32_t* first;
+  uint32_t* second;
+  hfb_contact* contacts;
+  uint32_t* n_env_candidates;
+  uint32_t* n_env_colliding;
+  uint32_t* n_self_candidates;
+  uint32_t* n_self_colliding;
+} hfb_motions_out;
+int hfb_env_collide_motions(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                            const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                            const hfb_collision_request* req, const hfb_motions_out* out);
+int hfb_env_collide_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, size_t links_per_config, size_t n_self_pairs,
+                                   const uint32_t* self_pairs, size_t n_motions, const uint32_t* motion_offsets,
+                                   size_t first_motion, size_t num_motions, const hfb_collision_request* req,
+                                   const hfb_motions_out* d_out, void* cuda_stream);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
