@@ -179,6 +179,13 @@ class MotionsOut(C.Structure):  # hfb_motions_out: per motion its first collidin
                 ("n_self_candidates", C.c_void_p), ("n_self_colliding", C.c_void_p)]
 
 
+class CertifyOut(C.Structure):  # hfb_certify_out: per motion its first colliding and first uncertified sample, per
+    # configuration whether the segment to the next sample is certified free
+    _fields_ = [("first_invalid", C.c_void_p), ("first_uncertified", C.c_void_p), ("certified", C.c_void_p),
+                ("n_env_candidates", C.c_void_p), ("n_self_candidates", C.c_void_p), ("n_unsupported", C.c_void_p),
+                ("n_uncertified", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -783,6 +783,26 @@ class ResidentEnvironment:
         return self.engine.env_collide_motions(self._env, h, t, links_per_config, tpl, off, req, first_motion,
                                                num_motions, witness=False)[0]
 
+    def certify_motions(self, robot_manager, links_per_config, self_pairs, motion_offsets, sweep, request=None,
+                        first_motion=0, num_motions=None):
+        """A planner's continuous motion validation: the motions of collide_motions(), and sweep (one float64 per
+        object of the robot manager): sweep[g * links_per_config + i] bounds the path length of every point of link i
+        from configuration g to g + 1 (hpp-core's maximal velocity times the step; not finite and >= 0: the segment is
+        not certified).  -> (first_invalid: per motion what collide_motions() returns; first_uncertified: per motion the
+        first segment not certified free, -1 when all are; certified: per configuration 1 when the segment to the next
+        sample of its motion is certified free).  A segment is certified when, at both its ends, every pair's collide()
+        lower bound exceeds half its sweep (include/hppfcl_b200.h, hfb_env_certify_motions, states the rule and its
+        guarantee).  Only motions [first_motion, first_motion + num_motions) are checked."""
+        h, t, req = self._robot(robot_manager, request)
+        tpl = self._template_args(links_per_config, self_pairs)
+        off, first_motion, num_motions = self._motion_args(len(h), links_per_config, motion_offsets, first_motion,
+                                                           num_motions)
+        sw = np.asarray(sweep, dtype=np.float64).reshape(-1)
+        if sw.shape[0] != len(h):
+            raise ValueError("sweep: one bound per object of the robot manager")
+        return self.engine.env_certify_motions(self._env, h, t, sw, links_per_config, tpl, off, req, first_motion,
+                                               num_motions)[:3]
+
     @staticmethod
     def _motion_args(n_objects, links_per_config, motion_offsets, first_motion, num_motions):
         """the offsets and the motion range as the C ABI takes them; ones the C ABI refuses raise ValueError (the C++

@@ -813,6 +813,116 @@ __global__ void __launch_bounds__(256) k_mot_final(BpMotions ms) {
   ms.first_invalid[m] = k == 0xffffffffu ? -1 : (int32_t)k;
 }
 
+// ---- hfb_env_certify_motions (BpCertify in hfb_broadphase.h) -------------------------------------------------------
+// one thread per A object of the range: its sides, and its box widened by its reach (the only place that knows where
+// the motions end; every later pass reads the sides)
+__global__ void __launch_bounds__(256) k_sweep_sides(const double* bb, const double* sweep, unsigned a_lo, unsigned a_hi,
+                                                     BpCertify c, double* wbb) {
+  const unsigned i = a_lo + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a_hi) return;
+  const unsigned m = motion_of(c.off, c.m0, c.m1, i / c.links);
+  double r, l;
+  sweep_sides(sweep, i, c.links, c.off[m], c.off[m + 1], &r, &l);
+  c.sides[2 * (size_t)i] = r;
+  c.sides[2 * (size_t)i + 1] = l;
+  const double* b = bb + 6 * (size_t)i;
+  double o[6];
+  if (aabb_empty(b)) {
+    for (int k = 0; k < 6; ++k) o[k] = b[k];
+  } else {
+    dist_inflate(b, sweep_reach(r, l), o);
+  }
+  for (int k = 0; k < 6; ++k) wbb[6 * (size_t)i + k] = o[k];
+}
+// the self candidates (sweep_pair): one thread per (configuration, template pair), as k_config_pairs
+__global__ void __launch_bounds__(128) k_sweep_pairs(const double* bb, BpCertify c, const uint32_t* tpl, unsigned n_tpl,
+                                                     size_t total, uint32_t* first, uint32_t* second, unsigned capacity,
+                                                     unsigned* n_pairs) {
+  const size_t tend = (total + 31u) & ~(size_t)31;  // (warp-uniform trip count for the ballots)
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < tend; t += (size_t)gridDim.x * blockDim.x) {
+    bool hit = false;
+    uint32_t a = 0, b = 0;
+    if (t < total) hit = sweep_pair(bb, c.sides, c.links, tpl, n_tpl, c.g0, t, &a, &b);
+    append_pair(hit, a, b, first, second, capacity, n_pairs);
+  }
+}
+// per configuration of the range: a side passes until a pair fails it, and exists when every link has it; per motion:
+// no colliding sample, no uncertified segment
+__global__ void __launch_bounds__(256) k_cert_init(BpCertify c, unsigned n_motions) {
+  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < c.ng) {
+    const double* s = c.sides + 2 * (size_t)(c.g0 + t) * c.links;
+    bool r = true, l = true;
+    for (unsigned i = 0; i < c.links; ++i) {
+      r = r && s[2 * i] == s[2 * i];  // (NaN: no side)
+      l = l && s[2 * i + 1] == s[2 * i + 1];
+    }
+    c.pass[2 * (size_t)t] = r;
+    c.pass[2 * (size_t)t + 1] = l;
+  }
+  if (t < n_motions) c.sample[t] = c.unc[t] = 0xffffffffu;
+}
+// the candidates of one collide() pass; the environment pairs' boxes are A's and B's unwidened ones
+struct CertItems {
+  const hfb_contact* r;
+  const uint32_t *pf, *ps;
+  const double *ba, *bb_b;
+  unsigned n, split, second_base;
+};
+// one thread per record: the pair's two thresholds from the sides clear its sample's flags unless the record clears
+// them (no contact, supported, 2 * lower bound above the threshold; NaN never does); a contact of a pair whose
+// unwidened boxes overlap makes its sample collide
+__global__ void __launch_bounds__(256) k_cert_pairs(BpCertify c, CertItems it, unsigned* n_unsupported) {
+  const unsigned p = blockIdx.x * blockDim.x + threadIdx.x;
+  bool unsup = false;
+  if (p < it.n) {
+    const hfb_contact& rec = it.r[p];
+    const bool env = p < it.split;
+    const uint32_t a = it.pf[p], b = env ? it.ps[p] - it.second_base : it.ps[p];
+    double sr = c.sides[2 * (size_t)a], sl = c.sides[2 * (size_t)a + 1];
+    if (!env) {
+      sr = add_ru(sr, c.sides[2 * (size_t)b]);
+      sl = add_ru(sl, c.sides[2 * (size_t)b + 1]);
+    }
+    unsup = ((rec.status >> 16) & 0xffu) == HFB_PATH_UNSUPPORTED;
+    const bool clear = rec.num_contacts == 0 && !unsup;
+    const double d2 = 2.0 * rec.distance_lower_bound;
+    const unsigned g = a / c.links;
+    uint8_t* f = c.pass + 2 * (size_t)(g - c.g0);
+    if (!(clear && d2 > sr)) f[0] = 0;
+    if (!(clear && d2 > sl)) f[1] = 0;
+    if (rec.num_contacts > 0 && aabb_overlap(it.ba + 6 * (size_t)a, (env ? it.bb_b : it.ba) + 6 * (size_t)b)) {
+      const unsigned m = motion_of(c.off, c.m0, c.m1, g);
+      atomicMin(c.sample + m, g - c.off[m]);
+    }
+  }
+  const unsigned mu = __ballot_sync(0xffffffffu, unsup);
+  if ((threadIdx.x & 31u) == 0 && mu) atomicAdd(n_unsupported, (unsigned)__popc(mu));
+}
+// per configuration of the range: certified when it has a successor in its motion (its right side exists), its right
+// side passes and its successor's left side passes; a motion's first segment that is not, and their count
+__global__ void __launch_bounds__(256) k_cert_final(BpCertify c, unsigned* n_uncertified) {
+  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+  bool unc = false;
+  if (t < c.ng) {
+    const unsigned g = c.g0 + t, m = motion_of(c.off, c.m0, c.m1, g);
+    const bool seg = g + 1 < c.off[m + 1];
+    const bool cert = seg && c.pass[2 * (size_t)t] && c.pass[2 * (size_t)t + 3];
+    if (c.certified) c.certified[t] = cert;
+    unc = seg && !cert;
+    if (unc) atomicMin(c.unc + m, g - c.off[m]);
+  }
+  const unsigned mu = __ballot_sync(0xffffffffu, unc);
+  if ((threadIdx.x & 31u) == 0 && mu) atomicAdd(n_uncertified, (unsigned)__popc(mu));
+}
+__global__ void __launch_bounds__(256) k_cert_motions(BpCertify c) {
+  const unsigned m = c.m0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= c.m1) return;
+  const unsigned k = c.sample[m], u = c.unc[m];
+  if (c.first_invalid) c.first_invalid[m] = k == 0xffffffffu ? -1 : (int32_t)k;
+  if (c.first_uncertified) c.first_uncertified[m] = u == 0xffffffffu ? -1 : (int32_t)u;
+}
+
 size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
 struct Scratch {
   Bounds* part;
@@ -1231,6 +1341,66 @@ int bp_motions_final_launch(const BpMotions& ms, cudaStream_t s, int* launches) 
   if (n == 0 || !ms.first_invalid) return 0;
   k_mot_final<<<(n + 255) / 256, 256, 0, s>>>(ms);
   *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+size_t bp_certify_bytes(size_t n, bool staged) { return (staged ? 4 : 2) * up256(n * 4); }
+
+BpCertify bp_certify_carve(void* p, size_t n, bool staged) {
+  unsigned char* c = static_cast<unsigned char*>(p);
+  BpCertify cs{};
+  cs.sample = reinterpret_cast<unsigned*>(c); c += up256(n * 4);
+  cs.unc = reinterpret_cast<unsigned*>(c); c += up256(n * 4);
+  if (!staged) return cs;
+  cs.first_invalid = reinterpret_cast<int32_t*>(c); c += up256(n * 4);
+  cs.first_uncertified = reinterpret_cast<int32_t*>(c);
+  return cs;
+}
+
+int bp_sweep_sides_launch(const double* d_bb, const double* d_sweep, size_t a_lo, size_t a_hi, const BpCertify& c,
+                          double* d_wbb, cudaStream_t s, int* launches) {
+  if (a_hi <= a_lo) return 0;
+  k_sweep_sides<<<(unsigned)((a_hi - a_lo + 255) / 256), 256, 0, s>>>(d_bb, d_sweep, (unsigned)a_lo, (unsigned)a_hi, c,
+                                                                      d_wbb);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_sweep_pairs_launch(const double* d_bb, const BpCertify& c, const uint32_t* d_tpl, size_t n_tpl, uint32_t* d_first,
+                          uint32_t* d_second, size_t capacity, unsigned* d_n_pairs, int num_sms, cudaStream_t s,
+                          int* launches) {
+  const size_t total = (size_t)c.ng * n_tpl;
+  if (total == 0) return 0;
+  if (num_sms < 1) num_sms = 1;
+  size_t nb = (total + 127) / 128;
+  if (nb > (size_t)num_sms * 16u) nb = (size_t)num_sms * 16u;
+  k_sweep_pairs<<<(unsigned)nb, 128, 0, s>>>(d_bb, c, d_tpl, (unsigned)n_tpl, total, d_first, d_second,
+                                             (unsigned)(capacity > 0xffffffffull ? 0xffffffffull : capacity), d_n_pairs);
+  *launches += 1;
+  return (int)cudaGetLastError();
+}
+
+int bp_certify_launch(const hfb_contact* d_recs, const uint32_t* d_first, const uint32_t* d_second, size_t n, size_t split,
+                      uint32_t second_base, const double* d_ba, const double* d_bb_b, const BpCertify& c,
+                      unsigned* d_counts, cudaStream_t s, int* launches) {
+  const unsigned n_motions = c.m1;  // (the state of motions [0, m1) is set: the range's binary search reads no other)
+  const unsigned n_init = c.ng > n_motions ? c.ng : n_motions;
+  if (n_init == 0) return 0;
+  k_cert_init<<<(n_init + 255) / 256, 256, 0, s>>>(c, n_motions);
+  *launches += 1;
+  if (n) {
+    const CertItems it{d_recs, d_first, d_second, d_ba, d_bb_b, (unsigned)n, (unsigned)split, second_base};
+    k_cert_pairs<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c, it, d_counts);
+    *launches += 1;
+  }
+  if (c.ng) {
+    k_cert_final<<<(c.ng + 255) / 256, 256, 0, s>>>(c, d_counts + 1);
+    *launches += 1;
+  }
+  if (c.m1 > c.m0) {
+    k_cert_motions<<<(c.m1 - c.m0 + 255) / 256, 256, 0, s>>>(c);
+    *launches += 1;
+  }
   return (int)cudaGetLastError();
 }
 

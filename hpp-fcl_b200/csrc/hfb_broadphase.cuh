@@ -523,4 +523,58 @@ inline size_t broadphase_config_distance_pairs_host(const double* bb, uint32_t l
   return count;
 }
 
+// ---- hfb_env_certify_motions: the sides of a sample and the candidates they widen -------------------------------
+// A side of sample g is the segment to g + 1 (right) or from g - 1 (left) of its motion; an object's side is the
+// caller's sweep bound of its link on that segment, NaN when the segment does not exist or the bound is not finite and
+// >= 0.  A NaN side widens nothing and fails every threshold test (a comparison with NaN is false).
+HFB_HD double sweep_side(double s) { return s >= 0 && s <= DBL_MAX ? s : NAN; }
+// s / 2 rounded up: exact but for subnormals
+HFB_HD double half_ru(double s) {
+#ifdef __CUDA_ARCH__
+  return __dmul_ru(s, 0.5);
+#else
+  const double h = s * 0.5;
+  return h + h < s ? nextafter(h, INFINITY) : h;
+#endif
+}
+// the widening of a link or pair whose side thresholds are r and l: half the larger one that is not NaN, rounded up;
+// 0 when both are NaN.  A pair whose boxes are more than this apart is farther apart than half of either threshold.
+HFB_HD double sweep_reach(double r, double l) {
+  double s = 0;
+  if (r > s) s = r;
+  if (l > s) s = l;
+  return half_ru(s);
+}
+// the motion of configuration g among motions [m0, m1): the last one starting at or before it (off[m0] <= g <
+// off[m1]; an empty motion starts where the next one does)
+HFB_HD unsigned motion_of(const uint32_t* off, unsigned m0, unsigned m1, size_t g) {
+  unsigned lo = m0, hi = m1;
+  while (hi - lo > 1) {
+    const unsigned mid = lo + (hi - lo) / 2;
+    if (off[mid] <= g) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+// the right and left sides of A object i = g * links + link, whose configuration g lies in the motion [g_lo, g_hi)
+HFB_HD void sweep_sides(const double* sweep, size_t i, size_t links, size_t g_lo, size_t g_hi, double* r, double* l) {
+  const size_t g = i / links;
+  *r = g + 1 < g_hi ? sweep_side(sweep[i]) : NAN;
+  *l = g > g_lo ? sweep_side(sweep[i - links]) : NAN;
+}
+// self pair t (config_pair's numbering), `sides` the right and left side of every A object: true when its collide()
+// runs for certification -- both links have a box, and config_dist_pair holds with the pair's reach (sweep_reach of
+// the sums of its links' sides, rounded up) in place of max_distance.  A pair it skips has a box gap larger than half
+// of either threshold.
+HFB_HD bool sweep_pair(const double* bb, const double* sides, uint32_t links, const uint32_t* tpl, uint32_t n_pairs,
+                       uint32_t g0, size_t t, uint32_t* a, uint32_t* b) {
+  const size_t g = g0 + t / n_pairs, k = t % n_pairs;
+  const size_t i = g * links + tpl[2 * k], j = g * links + tpl[2 * k + 1];
+  *a = (uint32_t)i;
+  *b = (uint32_t)j;
+  if (aabb_empty(bb + 6 * i) || aabb_empty(bb + 6 * j)) return false;
+  const double w = sweep_reach(add_ru(sides[2 * i], sides[2 * j]), add_ru(sides[2 * i + 1], sides[2 * j + 1]));
+  return config_dist_pair(bb, links, tpl, n_pairs, g0, t, w, a, b);
+}
+
 }  // namespace hfb

@@ -153,6 +153,42 @@ int bp_motions_reduce_launch(const hfb_contact* d_recs, const uint32_t* d_first,
                              cudaStream_t s, int* launches);
 // first_invalid of the motions checked from the state (-1: none)
 int bp_motions_final_launch(const BpMotions& ms, cudaStream_t s, int* launches);
+// ---- hfb_env_certify_motions: motions certified between their samples from lower bounds and sweeps (DESIGN.md §3) --
+// The sides of each A object (sweep_sides of hfb_broadphase.cuh) widen its box for the environment candidates and its
+// self pairs' boxes for the self candidates; the collide() records of the candidates then clear per-sample pass flags
+// (a pair passes a side when it has no contact, is supported and 2 * distance_lower_bound exceeds the side's
+// threshold), and the unwidened overlaps among them give the first colliding sample as hfb_env_collide_motions does.
+struct BpCertify {
+  const uint32_t* off;  // the motion offsets, n_motions + 1 (device copy)
+  unsigned m0, m1;      // the motions checked
+  unsigned links, g0, ng;  // their configurations: [g0, g0 + ng)
+  double* sides;        // 2 per A object: right side, left side (NaN: none)
+  uint8_t* pass;        // 2 per configuration of the range (index g - g0): every pair passes the right / left side
+  unsigned* sample;     // per motion: the smallest colliding sample, UINT32_MAX: none
+  unsigned* unc;        // per motion: the smallest uncertified segment, UINT32_MAX: none
+  int32_t* first_invalid;      // outputs, n_motions each (may be null)
+  int32_t* first_uncertified;
+  uint8_t* certified;   // per configuration of the range, index g - g0 (may be null)
+};
+// bytes of the per-motion state (sample, unc, and with `staged` the two per-motion outputs) and its carving
+size_t bp_certify_bytes(size_t n_motions, bool staged);
+BpCertify bp_certify_carve(void* p, size_t n_motions, bool staged);
+// the sides of A objects [a_lo, a_hi) (c.sides) from the caller's sweep bounds d_sweep, and their boxes d_bb widened
+// by their reach, rounded outward, into d_wbb (boxes without a box are copied)
+int bp_sweep_sides_launch(const double* d_bb, const double* d_sweep, size_t a_lo, size_t a_hi, const BpCertify& c,
+                          double* d_wbb, cudaStream_t s, int* launches);
+// the self candidates of the range's configurations (sweep_pair), APPENDED as bp_config_pairs_launch appends
+int bp_sweep_pairs_launch(const double* d_bb, const BpCertify& c, const uint32_t* d_tpl, size_t n_tpl, uint32_t* d_first,
+                          uint32_t* d_second, size_t capacity, unsigned* d_n_pairs, int num_sms, cudaStream_t s,
+                          int* launches);
+// the certification of the range from the n records d_recs of the candidates (environment pairs (i, second_base + j)
+// before `split`, self pairs from there on; n = 0: no records, every pair passes), d_ba / d_bb_b the unwidened boxes
+// of A and B: the per-sample flags and the per-motion state, then the outputs of c (first_invalid, first_uncertified:
+// motions [m0, m1) only; certified).  d_counts[0] += the records HFB_PATH_UNSUPPORTED, d_counts[1] += the range's
+// segments not certified.
+int bp_certify_launch(const hfb_contact* d_recs, const uint32_t* d_first, const uint32_t* d_second, size_t n, size_t split,
+                      uint32_t second_base, const double* d_ba, const double* d_bb_b, const BpCertify& c,
+                      unsigned* d_counts, cudaStream_t s, int* launches);
 // hfb_env_update: d_tfs[d_idx[k]] = d_tfs_new[k] and the box of object d_idx[k] recomputed, k < m
 int bp_env_update_launch(const double* d_local_aabbs, uint32_t nshapes, size_t m, const uint32_t* d_idx,
                          const hfb_transform* d_tfs_new, const uint32_t* d_handles, hfb_transform* d_tfs, double* d_aabbs,

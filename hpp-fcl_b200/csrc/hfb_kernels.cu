@@ -930,6 +930,8 @@ struct hfb_ctx {
   DevBuf sc_dist, sc_drec;  // hfb_env_distance: the per-A state (hfb::BpDistState), a round's distance() records
   DevBuf sc_cdist;          // hfb_env_distance_configs: the per-configuration state (hfb::BpConfigDist)
   DevBuf sc_moff, sc_mot;   // hfb_env_collide_motions: the motion offsets, the per-motion state (hfb::BpMotions)
+  DevBuf sc_sweep, sc_side, sc_cpass;  // hfb_env_certify_motions: the sweep bounds (host form), the sides and widened
+                                      // boxes of A, the per-sample pass flags (hfb::BpCertify)
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   uint64_t commits = 0, clears = 0;
@@ -2015,7 +2017,8 @@ void hfb_ctx_destroy(hfb_ctx* c) {
   for (cudaEvent_t e : c->pipe_events) cudaEventDestroy(e);
   c->bp_scratch.release();
   for (DevBuf* b : {&c->sc_bb, &c->sc_pf, &c->sc_ps, &c->sc_cnt, &c->sc_out, &c->sc_f, &c->sc_s, &c->sc_rec, &c->sc_flags,
-                    &c->sc_dist, &c->sc_drec, &c->sc_cdist})
+                    &c->sc_dist, &c->sc_drec, &c->sc_cdist, &c->sc_tpl, &c->sc_moff, &c->sc_mot, &c->sc_sweep,
+                    &c->sc_side, &c->sc_cpass})
     b->release();
   for (hfb_env* e : c->envs) delete e;
   c->obj_tf.release();
@@ -2804,6 +2807,42 @@ int hfb_broadphase_config_distance_pairs(size_t n_a, const double* aabbs, size_t
   return HFB_OK;
 }
 
+// the self pairs whose collide() hfb_env_certify_motions runs (sweep_pair), for the configurations of the motion range,
+// with the sides sweep_sides gives them
+int hfb_broadphase_sweep_pairs(size_t n_a, const double* aabbs, const double* sweep, size_t links_per_config,
+                               size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                               const uint32_t* motion_offsets, size_t first_motion, size_t num_motions, uint32_t* first,
+                               uint32_t* second, size_t capacity, size_t* n_pairs) {
+  if ((n_a && (!aabbs || !sweep)) || !n_pairs || (capacity && (!first || !second)) || (n_self_pairs && !self_pairs) ||
+      !motion_offsets || n_a > 0xffffffffull || n_self_pairs > 0xffffffffull || n_motions > 0xffffffffull)
+    return HFB_ERR_INVALID_ARGUMENT;
+  const size_t L = links_per_config;
+  const uint32_t* off = motion_offsets;
+  if (L == 0 || n_a % L || off[0] != 0 || off[n_motions] != n_a / L || first_motion > n_motions ||
+      num_motions > n_motions - first_motion || config_template_error(L, n_self_pairs, self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  for (size_t m = 0; m < n_motions; ++m)
+    if (off[m + 1] < off[m] || off[m + 1] - off[m] > 0x7fffffffu) return HFB_ERR_INVALID_ARGUMENT;
+  std::vector<double> sides(2 * n_a, std::numeric_limits<double>::quiet_NaN());
+  for (size_t m = first_motion; m < first_motion + num_motions; ++m)
+    for (size_t i = (size_t)off[m] * L; i < (size_t)off[m + 1] * L; ++i)
+      sweep_sides(sweep, i, L, off[m], off[m + 1], &sides[2 * i], &sides[2 * i + 1]);
+  const size_t g0 = off[first_motion], ng = off[first_motion + num_motions] - g0;
+  size_t count = 0;
+  for (size_t t = 0; t < ng * n_self_pairs; ++t) {
+    uint32_t a, b;
+    if (!sweep_pair(aabbs, sides.data(), (uint32_t)L, self_pairs, (uint32_t)n_self_pairs, (uint32_t)g0, t, &a, &b))
+      continue;
+    if (count < capacity) {
+      first[count] = a;
+      second[count] = b;
+    }
+    ++count;
+  }
+  *n_pairs = count;
+  return HFB_OK;
+}
+
 int hfb_broadphase_cross_pairs_device(hfb_ctx* ctx, size_t n_a, const double* d_aabbs_a, size_t first_a, size_t num_a,
                                       size_t n_b, const double* d_aabbs_b, uint32_t* d_first, uint32_t* d_second,
                                       size_t capacity, uint32_t* d_n_pairs, void* stream) {
@@ -3060,34 +3099,52 @@ static int configs_output(hfb_ctx* ctx, unsigned cand, unsigned split, uint32_t 
 // one candidate list -- the environment pairs against the built grid, then, after the split is noted in the counter's
 // second word, the self pairs appended to it -- and one narrow phase over the table [A; B].  entries: each self pair's
 // template entry in ctx->sc_f, at its position in the list.
+//
+// The general form: cross_boxes(d_bb, &boxes, &launches) gives the A boxes the grid query runs on (it may launch the
+// pass that makes them), and self_pairs(d_bb, pf, ps, cap, d_cnt, &launches) appends the self pairs; `entry` (may be
+// null) is a third candidate list, grown with the other two.
+template <class CrossBoxes, class SelfPairs>
 static int configs_candidates(hfb_ctx* ctx, hfb_env* e, size_t n_a, const ConfigTpl& t, const hfb_collision_request* req,
-                              bool minus_inf, bool entries, cudaStream_t s, unsigned* cand, unsigned* split) {
-  const size_t n_b = e->n_b, links = t.links, n_tpl = t.n, g0 = t.g0, ng = t.ng;
+                              bool minus_inf, DevBuf* entry, cudaStream_t s, unsigned* cand, unsigned* split,
+                              CrossBoxes cross_boxes, SelfPairs self_pairs) {
+  const size_t n_b = e->n_b, links = t.links, g0 = t.g0, ng = t.ng;
   const size_t a_lo = g0 * links, a_hi = (g0 + ng) * links;
   const BpCrossGrid g = bp_cross_grid_carve(e->grid.p, n_b);
   const double* bb_b = static_cast<const double*>(e->bb.p);
-  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
   CK(ctx->bp_scratch.reserve(bp_cross_scratch_bytes(n_a, n_b)));
   auto find = [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
-    int rc = 0;
+    const double* d_qb = nullptr;
+    int rc = cross_boxes(d_bb, &d_qb, nl);
+    if (rc) return rc;
     if (n_b) {
       rc = bp_cross_query_reset(g, d_cnt, s);
       if (!rc)
-        rc = bp_cross_query_launch(n_a, d_bb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
+        rc = bp_cross_query_launch(n_a, d_qb, a_lo, a_hi, n_b, bb_b, g, pf, ps, (uint32_t)n_a, cap, d_cnt,
                                    ctx->bp_scratch.p, ctx->num_sms, s, nl);
     } else {
       rc = (int)cudaMemsetAsync(d_cnt, 0, sizeof(unsigned), s);
     }
     if (!rc) rc = (int)cudaMemcpyAsync(d_cnt + 1, d_cnt, sizeof(unsigned), cudaMemcpyDeviceToDevice, s);
-    if (!rc)
-      rc = bp_config_pairs_launch(d_bb, links, d_tpl, n_tpl, g0, ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl,
-                                  entries ? static_cast<uint32_t*>(ctx->sc_f.p) : nullptr);
+    if (!rc) rc = self_pairs(d_bb, pf, ps, cap, d_cnt, nl);
     return rc;
   };
   const size_t off = e->head - n_a;
   return scene_candidates(ctx, s, n_a + n_b, static_cast<const uint32_t*>(e->h.p) + off,
-                          static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, cand, split,
-                          entries ? &ctx->sc_f : nullptr);
+                          static_cast<const hfb_transform*>(e->tf.p) + off, n_a, find, req, minus_inf, cand, split, entry);
+}
+static int configs_candidates(hfb_ctx* ctx, hfb_env* e, size_t n_a, const ConfigTpl& t, const hfb_collision_request* req,
+                              bool minus_inf, bool entries, cudaStream_t s, unsigned* cand, unsigned* split) {
+  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+  return configs_candidates(
+      ctx, e, n_a, t, req, minus_inf, entries ? &ctx->sc_f : nullptr, s, cand, split,
+      [](const double* d_bb, const double** d_qb, int*) {
+        *d_qb = d_bb;
+        return 0;
+      },
+      [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+        return bp_config_pairs_launch(d_bb, t.links, d_tpl, t.n, t.g0, t.ng, pf, ps, cap, d_cnt, ctx->num_sms, s, nl,
+                                      entries ? static_cast<uint32_t*>(ctx->sc_f.p) : nullptr);
+      });
 }
 
 // hfb_env_collide_configs: the candidates and their records (configs_candidates), then the outputs
@@ -3448,9 +3505,129 @@ struct EnvCollideMotions {
   }
 };
 
-// hfb_env_collide_motions' arguments beyond the pointers: the offsets, the motion range, then configs_args over the
-// range's configurations (into q.t)
-static int motions_args(hfb_ctx* ctx, size_t n_a, EnvCollideMotions& q) {
+// hfb_env_certify_motions' outputs, checked before the context is looked at
+static bool certify_ok(const hfb_certify_out* o) { return o && (o->first_invalid || o->first_uncertified || o->certified); }
+
+// hfb_env_certify_motions (the template in ctx->sc_tpl, the offsets in ctx->sc_moff, the sweep bounds in
+// ctx->sc_sweep in the host form): the sides of the range's A objects and their widened boxes (ctx->sc_side), the
+// candidates of the widened boxes and of sweep_pair with their collide() records (configs_candidates), then the
+// per-sample flags (ctx->sc_cpass) and the per-motion state (hfb::BpCertify, in ctx->sc_mot).  t.g0 and t.ng are set
+// by motions_args.
+struct EnvCertifyMotions {
+  const hfb_collision_request* req;
+  const hfb_certify_out* out;
+  ConfigTpl t;
+  size_t n_motions;
+  const uint32_t* offsets;
+  size_t first_motion, num_motions;
+  const double* sweep;
+  bool minus_inf = false;
+
+  const ConfigTpl* tpl() const { return &t; }
+  int check(hfb_ctx* ctx) { return collide_prelude(ctx, req, &minus_inf); }
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t n_a) const {
+    for (uint32_t* c : {out->n_env_candidates, out->n_self_candidates, out->n_unsupported, out->n_uncertified})
+      CK(o.zero(c, sizeof(uint32_t)));
+    CK(o.zero(out->certified, n_a / t.links));
+    const size_t n = n_motions;
+    if (o.dev) {  // (on the caller's stream: -1 for every motion)
+      int nl = 0;
+      for (int32_t* p : {out->first_invalid, out->first_uncertified}) {
+        BpMotions ms{};
+        ms.first_invalid = p;
+        if (p && bp_motions_init_launch(n, ms, o.s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_mot_init launch failed");
+      }
+      ctx->stats.kernel_launches += (uint64_t)nl;
+      return HFB_OK;
+    }
+    if (out->first_invalid) std::fill(out->first_invalid, out->first_invalid + n, -1);
+    if (out->first_uncertified) std::fill(out->first_uncertified, out->first_uncertified + n, -1);
+    return HFB_OK;
+  }
+  // (with no pair at all the segments with valid sweeps are still certified: only an empty range is empty)
+  bool empty(const hfb_env*, size_t n_a) const { return n_a == 0 || t.ng == 0; }
+  int run(hfb_ctx* ctx, hfb_env* e, size_t n_a, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const size_t n = n_motions, links = t.links;
+    CK(ctx->sc_moff.reserve((n + 1) * 4));
+    CK(cudaMemcpyAsync(ctx->sc_moff.p, offsets, (n + 1) * 4, cudaMemcpyHostToDevice, s));
+    const double* d_sweep = sweep;
+    if (!o.dev) {
+      CK(ctx->sc_sweep.reserve(n_a * 8));
+      CK(cudaMemcpyAsync(ctx->sc_sweep.p, sweep, n_a * 8, cudaMemcpyHostToDevice, s));
+      d_sweep = static_cast<const double*>(ctx->sc_sweep.p);
+    }
+    CK(ctx->sc_side.reserve(n_a * 64));  // per A object: its two sides (16 bytes), its widened box (48)
+    CK(ctx->sc_cpass.reserve(t.ng * 2));
+    CK(ctx->sc_mot.reserve(bp_certify_bytes(n, !o.dev)));
+    BpCertify c = bp_certify_carve(ctx->sc_mot.p, n, !o.dev);  // (the host form stages its outputs there)
+    c.off = static_cast<const uint32_t*>(ctx->sc_moff.p);
+    c.m0 = (unsigned)first_motion;
+    c.m1 = (unsigned)(first_motion + num_motions);
+    c.links = (unsigned)links;
+    c.g0 = (unsigned)t.g0;
+    c.ng = (unsigned)t.ng;
+    c.sides = static_cast<double*>(ctx->sc_side.p);
+    double* d_wbb = c.sides + 2 * n_a;
+    c.pass = static_cast<uint8_t*>(ctx->sc_cpass.p);
+    if (o.dev) {
+      c.first_invalid = out->first_invalid;
+      c.first_uncertified = out->first_uncertified;
+      c.certified = out->certified ? out->certified + t.g0 : nullptr;
+    } else {
+      if (!out->first_invalid) c.first_invalid = nullptr;
+      if (!out->first_uncertified) c.first_uncertified = nullptr;
+      if (out->certified) {
+        CK(ctx->sc_flags.reserve(t.ng));
+        c.certified = static_cast<uint8_t*>(ctx->sc_flags.p);
+      }
+    }
+    const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+    const size_t a_lo = t.g0 * links, a_hi = (t.g0 + t.ng) * links;
+    bool sided = false;  // (the finder runs twice when the candidate lists grow; the sides are made once)
+    unsigned cand = 0, split = 0;
+    if (int rc = configs_candidates(
+            ctx, e, n_a, t, req, minus_inf, nullptr, s, &cand, &split,
+            [&](const double* d_bb, const double** d_qb, int* nl) {
+              *d_qb = d_wbb;
+              if (sided) return 0;
+              sided = true;
+              return bp_sweep_sides_launch(d_bb, d_sweep, a_lo, a_hi, c, d_wbb, s, nl);
+            },
+            [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+              return bp_sweep_pairs_launch(d_bb, c, d_tpl, t.n, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
+            }))
+      return rc;
+    CK(o.count(out->n_env_candidates, split));
+    CK(o.count(out->n_self_candidates, cand - split));
+    unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+    CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
+    // under minus_inf no record exists (collision.cpp:73-76): every pair passes, every sample is valid
+    const size_t n_recs = minus_inf ? 0 : cand;
+    int nl = 0;
+    if (bp_certify_launch(static_cast<const hfb_contact*>(ctx->sc_out.p), static_cast<const uint32_t*>(ctx->sc_pf.p),
+                          static_cast<const uint32_t*>(ctx->sc_ps.p), n_recs, split, (uint32_t)n_a,
+                          static_cast<const double*>(ctx->sc_bb.p), static_cast<const double*>(e->bb.p), c, d_cnt + 1, s,
+                          &nl) != 0)
+      return fail(ctx, HFB_ERR_CUDA, "k_cert_pairs launch failed");
+    ctx->stats.kernel_launches += (uint64_t)nl;
+    if (!o.dev) {
+      const size_t m0 = first_motion, nm = num_motions;
+      if (out->first_invalid) CK(o.copy(out->first_invalid + m0, c.first_invalid + m0, nm * 4));
+      if (out->first_uncertified) CK(o.copy(out->first_uncertified + m0, c.first_uncertified + m0, nm * 4));
+      if (out->certified) CK(o.copy(out->certified + t.g0, c.certified, t.ng));
+    }
+    CK(o.copy(out->n_unsupported, d_cnt + 1, sizeof(unsigned)));
+    CK(o.copy(out->n_uncertified, d_cnt + 2, sizeof(unsigned)));
+    CK(o.finish());
+    return HFB_OK;
+  }
+};
+
+// hfb_env_collide_motions' and hfb_env_certify_motions' arguments beyond the pointers: the offsets, the motion range,
+// then configs_args over the range's configurations (into q.t)
+template <class MotionsQuery>
+static int motions_args(hfb_ctx* ctx, size_t n_a, MotionsQuery& q) {
   const size_t links = q.t.links, n = q.n_motions;
   const uint32_t* off = q.offsets;
   if (links == 0 || n_a % links) return fail(ctx, HFB_ERR_INVALID_ARGUMENT, "n_a is not a multiple of links_per_config");
@@ -3475,6 +3652,7 @@ static int query_args(hfb_ctx* ctx, size_t n_a, Query& q) {
   return t ? configs_args(ctx, n_a, t->links, t->n, t->pairs, t->g0, t->ng) : HFB_OK;
 }
 static int query_args(hfb_ctx* ctx, size_t n_a, EnvCollideMotions& q) { return motions_args(ctx, n_a, q); }
+static int query_args(hfb_ctx* ctx, size_t n_a, EnvCertifyMotions& q) { return motions_args(ctx, n_a, q); }
 
 // The frame of the hfb_env_* queries (EnvCollide, EnvCollideConfigs, EnvDistance, EnvDistanceConfigs), with their
 // pointers checked: the lock, the query's and the env's checks, A uploaded into the env's table in front of B (and
@@ -3663,6 +3841,35 @@ int hfb_env_collide_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
   return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
                   EnvCollideMotions{req, d_out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
                                     motion_offsets, first_motion, num_motions});
+}
+
+// A planner's continuous motion validation (hfb_certify_out in include/hppfcl_b200.h): hfb_env_collide_motions'
+// first colliding sample per motion, and each segment between consecutive samples certified free from the collide()
+// lower bounds of its two end samples and the caller's sweep bounds -- hpp-core's continuous path validation
+// (BodyPairCollision's interval from CollisionResult::distance_lower_bound and the maximal velocity).
+int hfb_env_certify_motions(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            const double* sweep, size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs,
+                            size_t n_motions, const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                            const hfb_collision_request* req, const hfb_certify_out* out) {
+  if (!ctx || !env || !req || !certify_ok(out) || !motion_offsets || !sweep || (n_a && (!handles_a || !tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::host, nullptr, n_a, handles_a, tfs_a,
+                  EnvCertifyMotions{req, out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
+                                    motion_offsets, first_motion, num_motions, sweep});
+}
+
+int hfb_env_certify_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, const double* d_sweep, size_t links_per_config,
+                                   size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                                   const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                                   const hfb_collision_request* req, const hfb_certify_out* d_out, void* stream) {
+  if (!ctx || !env || !req || !certify_ok(d_out) || !motion_offsets || !d_sweep || (n_a && (!d_handles_a || !d_tfs_a)) ||
+      (n_self_pairs && !self_pairs))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
+                  EnvCertifyMotions{req, d_out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
+                                    motion_offsets, first_motion, num_motions, d_sweep});
 }
 
 // Each A object's nearest B object (hfb_env_distance_out in include/hppfcl_b200.h): the result of

@@ -81,6 +81,9 @@ def load_library(path=None):
     L.hfb_env_collide_motions.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp]
     L.hfb_env_collide_motions_device.argtypes = [vp, vp, sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, vp]
     L.hfb_broadphase_config_distance_pairs.argtypes = [sz, vp, sz, sz, vp, sz, sz, C.c_double, vp, vp, sz, vp]
+    L.hfb_env_certify_motions.argtypes = [vp, vp, sz, vp, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp]
+    L.hfb_env_certify_motions_device.argtypes = [vp, vp, sz, vp, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, vp]
+    L.hfb_broadphase_sweep_pairs.argtypes = [sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, sz, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -206,6 +209,37 @@ def broadphase_config_distance_pairs(aabbs, links_per_config, self_pairs, max_di
                                                 C.byref(cnt))
     if rc != 0:
         raise EngineError("hfb_broadphase_config_distance_pairs: %s" % _ERR.get(rc, rc))
+    k = min(cnt.value, cap)
+    return first[:k], second[:k]
+
+
+def broadphase_sweep_pairs(aabbs, sweep, links_per_config, self_pairs, offsets, first_motion=0, num_motions=None,
+                           capacity=None):
+    """the self pairs whose collide() the motion certification runs: boxes (n x 6) and sweep bounds (n) of n_configs x
+    links_per_config objects, configuration-major, motion m being configurations [offsets[m], offsets[m+1]); for every
+    configuration g of the motion range and template pair (i, j), (g * L + i, g * L + j) when both boxes exist and,
+    unless both are finite, j's box overlaps i's box widened by the pair's reach: half the larger of its right and left
+    thresholds (the sums of its links' sweeps, rounded up), rounded up (hfb_broadphase_sweep_pairs) -> (first, second),
+    configuration by configuration in template order.  Host function of the library: needs neither a context nor a
+    GPU."""
+    L = load_library()
+    bb = np.ascontiguousarray(aabbs, dtype=np.float64).reshape(-1, 6)
+    sw = np.ascontiguousarray(sweep, dtype=np.float64).reshape(-1)
+    tpl = _template(self_pairs)
+    off = _offsets(offsets)
+    n, lpc, n_motions = bb.shape[0], int(links_per_config), off.shape[0] - 1
+    if sw.shape[0] != n:
+        raise ValueError("sweep: one bound per object")
+    if num_motions is None:
+        num_motions = n_motions - first_motion
+    cap = int(capacity) if capacity is not None else max(tpl.shape[0] * (n // lpc if lpc else 0), 1)
+    first = np.empty(max(cap, 1), dtype=np.uint32)
+    second = np.empty(max(cap, 1), dtype=np.uint32)
+    cnt = C.c_size_t(0)
+    rc = L.hfb_broadphase_sweep_pairs(n, _ptr(bb), _ptr(sw), lpc, tpl.shape[0], _ptr(tpl), n_motions, _ptr(off),
+                                      int(first_motion), int(num_motions), _ptr(first), _ptr(second), cap, C.byref(cnt))
+    if rc != 0:
+        raise EngineError("hfb_broadphase_sweep_pairs: %s" % _ERR.get(rc, rc))
     k = min(cnt.value, cap)
     return first[:k], second[:k]
 
@@ -659,6 +693,51 @@ class Engine:
         self._check(self.L.hfb_env_collide_motions_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a),
                                                           int(links_per_config), tpl.shape[0], _ptr(tpl), n_motions,
                                                           _ptr(off), first_motion,
+                                                          n_motions - first_motion if num_motions is None else num_motions,
+                                                          C.byref(req), C.byref(out), _ptr(stream)))
+
+    def env_certify_motions(self, env, handles_a, tfs_a, sweep, links_per_config, self_pairs, offsets, req=None,
+                            first_motion=0, num_motions=None):
+        """motions of configurations laid out as in env_collide_motions, each segment between consecutive samples
+        certified free from the collide() lower bounds of its end samples and the sweep bounds (sweep: n_a float64,
+        sweep[g * L + i] bounding link i's points' path from configuration g to g + 1; hfb_env_certify_motions) ->
+        (first_invalid: per motion the first colliding sample, -1 for none; first_uncertified: per motion the first
+        segment not certified, -1 for none; certified: per configuration 1 when the segment to the next sample is;
+        counts = (n_env_candidates, n_self_candidates, n_unsupported, n_uncertified))"""
+        req = req or P.CollisionRequestPOD()
+        ha, ta = self._objects(handles_a, tfs_a)
+        sw = np.ascontiguousarray(sweep, dtype=np.float64).reshape(-1)
+        if sw.shape[0] != ha.shape[0]:
+            raise ValueError("sweep: one bound per object of A")
+        tpl = _template(self_pairs)
+        off = _offsets(offsets)
+        na, n_motions, lpc = ha.shape[0], off.shape[0] - 1, int(links_per_config)
+        first_invalid = np.empty(n_motions, dtype=np.int32)
+        first_uncertified = np.empty(n_motions, dtype=np.int32)
+        certified = np.empty(na // lpc if lpc else 0, dtype=np.uint8)
+        nc = np.zeros(4, dtype=np.uint32)
+        out = P.CertifyOut(first_invalid.ctypes.data, first_uncertified.ctypes.data, certified.ctypes.data,
+                           *[nc[k:].ctypes.data for k in range(4)])
+        self._check(self.L.hfb_env_certify_motions(self.h, env, na, _ptr(ha), _ptr(ta), _ptr(sw), lpc, tpl.shape[0],
+                                                   _ptr(tpl), n_motions, _ptr(off), first_motion,
+                                                   n_motions - first_motion if num_motions is None else num_motions,
+                                                   C.byref(req), C.byref(out)))
+        return first_invalid, first_uncertified, certified, tuple(int(c) for c in nc)
+
+    def env_certify_motions_device(self, env, n_a, d_handles_a, d_tfs_a, d_sweep, links_per_config, self_pairs, offsets,
+                                   d_first_invalid, d_first_uncertified, d_certified, d_counts=(None,) * 4, req=None,
+                                   stream=0, first_motion=0, num_motions=None):
+        """hfb_env_certify_motions_device: A's handles and poses, the sweep bounds and every output are device
+        pointers, ordered on `stream`; d_counts = (d_n_env_candidates, d_n_self_candidates, d_n_unsupported,
+        d_n_uncertified); the template and the offsets are host arrays"""
+        req = req or P.CollisionRequestPOD()
+        tpl = _template(self_pairs)
+        off = _offsets(offsets)
+        n_motions = off.shape[0] - 1
+        out = P.CertifyOut(d_first_invalid, d_first_uncertified, d_certified, *d_counts)
+        self._check(self.L.hfb_env_certify_motions_device(self.h, env, n_a, _ptr(d_handles_a), _ptr(d_tfs_a),
+                                                          _ptr(d_sweep), int(links_per_config), tpl.shape[0], _ptr(tpl),
+                                                          n_motions, _ptr(off), first_motion,
                                                           n_motions - first_motion if num_motions is None else num_motions,
                                                           C.byref(req), C.byref(out), _ptr(stream)))
 

@@ -1108,6 +1108,44 @@ class ResidentEnvironment {
     return first_invalid;
   }
 
+  /// A planner's continuous motion validation: the motions of collide_motions, and sweep (one bound per robot object):
+  /// sweep[g * links_per_config + i] bounds the path length of every point of link i from configuration g to g + 1
+  /// (hpp-core's maximal velocity times the step; not finite and >= 0: the segment is not certified).  Per motion:
+  /// first_invalid[m], what collide_motions gives; first_uncertified[m], the first segment not certified free (-1 when
+  /// all are); returns per configuration 1 when the segment to the next sample of its motion is certified free
+  /// (hfb_env_certify_motions states the rule and its guarantee).  A sweep whose size is not the robot's, malformed
+  /// offsets or a malformed template throw std::invalid_argument.
+  std::vector<uint8_t> certify_motions(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
+                                       const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs,
+                                       const std::vector<uint32_t>& offsets, const std::vector<double>& sweep,
+                                       const CollisionRequest& request, std::vector<int32_t>& first_invalid,
+                                       std::vector<int32_t>& first_uncertified) {
+    if (offsets.empty()) throw std::invalid_argument("motion offsets: n_motions + 1 values, at least one");
+    if (sweep.size() != robot.hs.size()) throw std::invalid_argument("sweep: one bound per object of the robot manager");
+    const size_t n = offsets.size() - 1;
+    first_invalid.resize(n);
+    first_uncertified.resize(n);
+    std::vector<uint8_t> certified(links_per_config ? robot.hs.size() / links_per_config : 0);
+    hfb_collision_request q;
+    prepare(robot, request, q);
+    std::vector<uint32_t> tpl;
+    for (const auto& p : self_pairs) {
+      tpl.push_back(p.first);
+      tpl.push_back(p.second);
+    }
+    // empty vectors may hand out null data(), which the C ABI would take for outputs not asked for (or a missing
+    // sweep); one slot stands in (nothing is read from or written to it)
+    int32_t none = -1;
+    double no_sweep = 0;
+    hfb_certify_out o{first_invalid.data(), first_uncertified.data(), certified.data(), nullptr, nullptr, nullptr,
+                      nullptr};
+    if (n == 0) o.first_invalid = &none;
+    C.check(hfb_env_certify_motions(C.raw(), env, robot.hs.size(), robot.hs.data(), robot.tfs.data(),
+                                    sweep.empty() ? &no_sweep : sweep.data(), links_per_config, self_pairs.size(),
+                                    tpl.data(), n, offsets.data(), 0, n, &q, &o));
+    return certified;
+  }
+
  private:
   void check_motions(DynamicAABBTreeCollisionManager& robot, size_t links_per_config,
                      const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, const std::vector<uint32_t>& offsets,

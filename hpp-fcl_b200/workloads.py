@@ -389,6 +389,56 @@ def robot_motions(n_motions, n_links=16, n_env=100_000, room=None, seed=0xFC1 + 
     return w
 
 
+def chain_sweep_bounds(w):
+    """Sweep bounds for robot_motions' chain, as hfb_env_certify_motions takes them: (n_configs * n_links,) float64,
+    entry g * L + l bounding the path length of every point of link l from sample g to sample g + 1 of its motion, 0 at
+    a motion's last sample (never read there).
+
+    Joint k turns about an axis through p_k, the start of link k (joint 0, the base yaw, through the base).  Every point
+    of link l >= k lies within rho_{k,l} = (l - k + 1) * link_len + 0.06 of p_k: l - k links of length link_len up to
+    p_l, then link l itself, whose points lie within link_len along its axis and, across it, within the box corner
+    0.04 * sqrt(2) < 0.06 (capsules 0.035, hulls 0.05).  A point's speed is at most the sum over the joints below it
+    of |dq_k/dt| times its distance to joint k's axis, which is at most its distance to p_k.  The samples are linear
+    in q, so over a segment the path length of link l's points is at most
+    s_{g,l} = sum_{k <= l} |q_{g+1,k} - q_{g,k}| * rho_{k,l}; it is computed in float64 and rounded up by a relative
+    margin far above the sum's rounding error."""
+    q, off, L, ll = np.asarray(w["q"], dtype=np.float64), np.asarray(w["offsets"], dtype=np.int64), w["n_links"], w["link_len"]
+    n = q.shape[0]
+    dq = np.zeros_like(q)
+    dq[:-1] = np.abs(q[1:] - q[:-1])
+    dq[off[1:][off[1:] > 0] - 1] = 0.0  # a motion's last sample (the next row is another motion's)
+    k, l = np.meshgrid(np.arange(L), np.arange(L), indexing="ij")
+    rho = np.where(k <= l, (l - k + 1) * ll + 0.06, 0.0)
+    s = dq @ rho
+    s = np.nextafter(s * (1.0 + 64 * L * np.finfo(np.float64).eps), np.inf)
+    s[dq.sum(axis=1) == 0] = 0.0
+    return np.ascontiguousarray(s.reshape(n * L))
+
+
+def resample_motions(w, configs, n_interior):
+    """the poses of robot_motions' chain at n_interior evenly spaced interior points of each segment from configuration
+    g to g + 1, g in `configs` (each with a successor in its motion): linear in q, through the same forward kinematics
+    -> transforms, n_interior * n_links per segment, segment after segment"""
+    L, ll = w["n_links"], w["link_len"]
+    g = np.asarray(configs, dtype=np.int64)
+    tf0 = w["tf_a"][g * L]  # link 0 of each start sample: its start is the base
+    base = tf0["T"] - 0.5 * ll * tf0["R"].reshape(-1, 3, 3)[:, 2, :]
+    t = np.arange(1, n_interior + 1) / (n_interior + 1.0)
+    q = w["q"][g][:, None, :] + t[None, :, None] * (w["q"][g + 1] - w["q"][g])[:, None, :]
+    base = np.repeat(base, n_interior, axis=0)
+    q = q.reshape(-1, L)
+    R = np.broadcast_to(np.eye(3), (len(q), 3, 3))
+    p = base.copy()
+    Rs, Ts = np.empty((len(q), L, 3, 3)), np.empty((len(q), L, 3))
+    for k in range(L):
+        R = R @ _axis_rotations(2 if k % 2 == 0 else 1, q[:, k])
+        axis = R[:, :, 2]
+        Rs[:, k] = R
+        Ts[:, k] = p + 0.5 * ll * axis
+        p = p + ll * axis
+    return P.make_transforms(Rs.reshape(-1, 3, 3), Ts.reshape(-1, 3))
+
+
 def chain_self_pairs(n_links, skip=2):
     """the self-pair template of a chain: every link pair (i, j) with j >= i + skip (neighbours touch at their joint
     and are not checked, as an SRDF disables adjacent links) -> (P, 2) uint32; 105 pairs for 16 links"""

@@ -686,6 +686,84 @@ int hfb_env_collide_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
                                    size_t first_motion, size_t num_motions, const hfb_collision_request* req,
                                    const hfb_motions_out* d_out, void* cuda_stream);
 
+/* ---- a planner's continuous motion validation: each segment between two samples certified free -------------------
+ * A, the template, the offsets, the motion range and the request are those of hfb_env_collide_motions, checked the
+ * same way; the template and the offsets stay in HOST memory in both forms.  sweep holds n_a doubles (host memory in
+ * the host form, device memory in the device form): sweep[g*L + i] is the caller's bound on the path length of every
+ * point of link i from configuration g to configuration g+1, samples k and k+1 of one motion (hpp-core's
+ * maximalVelocity times the step; the library does not interpolate).  The entry at a motion's last sample is never
+ * read.  A value that is not finite and >= 0 (NaN, negative, +-inf) is not an error: it widens nothing, and every
+ * segment it bounds is uncertified.
+ * Sides.  At sample g a pair has a right threshold (segment g -> g+1) and a left one (g-1 -> g): an environment pair
+ * (link i, B object j) has s_R = sweep[g*L+i] and s_L = sweep[(g-1)*L+i] (the environment does not move); a self pair
+ * (i, j) has s_R = sweep[g*L+i] + sweep[g*L+j] rounded up, and s_L the same at g-1.  A side exists when g has a
+ * successor (right) or predecessor (left) in its motion and its sweep values are valid.  A pair passes a side when the
+ * side exists, its collide() record has num_contacts == 0, its status is not HFB_PATH_UNSUPPORTED (whose cleared record
+ * carries distance_lower_bound = DBL_MAX) and 2 * distance_lower_bound > s (strict; NaN never passes).  A sample passes
+ * a side when every candidate pair of it does.
+ * Candidates.  w, the reach of a link or pair, is half the larger of its valid side thresholds, rounded up (0 with
+ * none).  Environment candidates: link i's box widened by w, rounded outward, overlaps B's box (the grid query runs on
+ * the widened boxes).  Self candidates: both links have a box, and unless both boxes are finite and link j's box does
+ * not overlap link i's box widened by w, rounded outward (hfb_broadphase_sweep_pairs).  A pair that is not a candidate
+ * passes both sides: its box gap, and so its distance, exceeds w.  At w = 0 the candidates include those of
+ * hfb_env_collide_configs.  Objects without a box take no part.  Every candidate runs collide() with the caller's
+ * request; its record is byte for byte what hfb_batch_collide_objects gives for that pair over the table [A; B].
+ * Outputs, per motion m and configuration g:
+ *   first_invalid[m]:     exactly what hfb_env_collide_motions returns: a sample collides iff one of its pairs whose
+ *                         unwidened boxes overlap has contacts.  A contact of a pair found by the widening alone (e.g.
+ *                         under a positive security_margin) does not invalidate the sample; it fails certification.
+ *   certified[g]:         1 iff g and g+1 are samples k and k+1 of one motion of the range, g's right side passes and
+ *                         g+1's left side passes; else 0 (a motion's last sample, configurations outside the range).
+ *                         n_configs bytes.
+ *   first_uncertified[m]: the smallest k with certified[offsets[m]+k] == 0 among the motion's n-1 segments, or -1
+ *                         (empty and one-sample motions, motions outside the range).
+ *   n_env_candidates, n_self_candidates: the widened candidates of the range; n_unsupported: the candidates that came
+ *   back HFB_PATH_UNSUPPORTED; n_uncertified: the range's segments with certified = 0.  32-bit counts, may be null.
+ *   first_invalid, first_uncertified and certified may each be null, but not all three.
+ * security_margin == -inf: no collide() runs, every motion is valid and every segment with valid sweeps certified.
+ * The guarantee.  If every point of each link travels at most its sweep along segment k and every
+ * distance_lower_bound used is a true lower bound, no pair of the segment touches anywhere inside it: after a fraction
+ * tau of the joint motion a pair's distance has dropped by at most (s_a + s_b) * tau from sample k, and by at most the
+ * rest from sample k+1, so passing both half-tests covers tau in [0, 1/2] from the left end and [1/2, 1] from the
+ * right.  For shape-shape leaves the reference subtracts security_margin from the lower bound: under a positive margin
+ * the pair also stays outside the margin; under a negative one the lower bound exceeds the true distance by |margin|,
+ * so the guarantee weakens to "no pair penetrates deeper than |margin|" (BVH pairs are unsupported there).  For GJK
+ * pairs the reference's lower bound is the converged distance, good to
+ * gjk_tolerance only: a caller who wants strict slack adds 2 * gjk_tolerance to each sweep.
+ * Refinement is the caller's: resample the segments with certified = 0 and call again (hpp-core's progressive
+ * validation).  Handles, the env's validity and the request are checked as hfb_env_collide checks them.  A refused
+ * call (a null sweep or output, all three per-item outputs null, or a refusal of hfb_env_collide_motions) writes
+ * nothing.
+ *   hfb_env_certify_motions: HOST buffers, blocking.
+ *   hfb_env_certify_motions_device: A's handles and poses, sweep and every output in DEVICE memory, ordered on
+ *     `cuda_stream`; it blocks where hfb_env_collide_motions_device does.  Later host calls on the context wait for it.
+ * hfb_broadphase_sweep_pairs: the self candidates above on the host (no context), for the configurations of the
+ * motion range, from the boxes `aabbs` (n_a x 6, as hfb_scene_aabbs writes them) and the sweep bounds; configuration
+ * by configuration in template order, all counted in *n_pairs, at most `capacity` stored.  Arguments are checked as
+ * hfb_env_certify_motions checks them. */
+typedef struct hfb_certify_out {
+  int32_t* first_invalid;     /* n_motions */
+  int32_t* first_uncertified; /* n_motions */
+  uint8_t* certified;         /* n_configs */
+  uint32_t* n_env_candidates;
+  uint32_t* n_self_candidates;
+  uint32_t* n_unsupported;
+  uint32_t* n_uncertified;
+} hfb_certify_out;
+int hfb_env_certify_motions(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* handles_a, const hfb_transform* tfs_a,
+                            const double* sweep, size_t links_per_config, size_t n_self_pairs, const uint32_t* self_pairs,
+                            size_t n_motions, const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                            const hfb_collision_request* req, const hfb_certify_out* out);
+int hfb_env_certify_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const uint32_t* d_handles_a,
+                                   const hfb_transform* d_tfs_a, const double* d_sweep, size_t links_per_config,
+                                   size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                                   const uint32_t* motion_offsets, size_t first_motion, size_t num_motions,
+                                   const hfb_collision_request* req, const hfb_certify_out* d_out, void* cuda_stream);
+int hfb_broadphase_sweep_pairs(size_t n_a, const double* aabbs, const double* sweep, size_t links_per_config,
+                               size_t n_self_pairs, const uint32_t* self_pairs, size_t n_motions,
+                               const uint32_t* motion_offsets, size_t first_motion, size_t num_motions, uint32_t* first,
+                               uint32_t* second, size_t capacity, size_t* n_pairs);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
