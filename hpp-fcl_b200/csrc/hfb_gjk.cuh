@@ -121,10 +121,44 @@ HFB_HD v3 ray_segment(v3 A, v3 X, v3 AX, double t) {
 // originToTriangle (:517-541), ABCdotAO != 0
 HFB_HD v3 ray_triangle(v3 N, double NdotAO) { return (-NdotAO / sqn(N)) * N; }
 
+// The new ray as a projection leaves it.  With DEFER (the default variant's GJK passes) a segment's or a face's ray is
+// not formed by the projection but left in `r`: ray_segment(A, X, X - A, t) (every segment's AX is X - A, the same
+// operation on the same values) or ray_triangle(N = A, NdotAO = t), which gjk_step evaluates after the projection of
+// every rank, so that a warp whose lanes project simplices of different ranks runs each formula, and its divisions,
+// once.  Without DEFER the projection forms the ray itself (the other kernels: carrying the inputs costs them more in
+// registers than it saves).  A vertex or a zero ray is always set in g.ray at once.
+enum { RAY_SET = 0, RAY_SEGMENT, RAY_TRIANGLE };
+struct RayOf {
+  int kind;
+  v3 A, X;
+  double t;
+};
+template <bool DEFER, class V>
+HFB_HD void ray_of_segment(GjkStateT<V>& g, RayOf& r, v3 A, v3 X, double t) {
+  if (!DEFER) {
+    g.ray = ray_segment(A, X, X - A, t);
+    return;
+  }
+  r.kind = RAY_SEGMENT;
+  r.A = A;
+  r.X = X;
+  r.t = t;
+}
+template <bool DEFER, class V>
+HFB_HD void ray_of_triangle(GjkStateT<V>& g, RayOf& r, v3 N, double NdotAO) {
+  if (!DEFER) {
+    g.ray = ray_triangle(N, NdotAO);
+    return;
+  }
+  r.kind = RAY_TRIANGLE;
+  r.A = N;
+  r.t = NdotAO;
+}
+
 // The projections read only w of each vertex and move whole vertices (V: SV or SVSlot).
 // projectLineOrigin (:543-569). A = newest = s1, B = s0.
-template <class V>
-HFB_HD bool project_line(GjkStateT<V>& g) {
+template <bool DEFER, class V>
+HFB_HD bool project_line(GjkStateT<V>& g, RayOf& r) {
   const v3 A = g.s1.w, B = g.s0.w;
   const v3 AB = B - A;
   const double d = dot(AB, -A);
@@ -138,14 +172,14 @@ HFB_HD bool project_line(GjkStateT<V>& g) {
     g.s0 = g.s1;
     g.rank = 1;
   } else {
-    g.ray = ray_segment(A, B, AB, d);  // next = [b, a]: order unchanged
+    ray_of_segment<DEFER>(g, r, A, B, d);  // next = [b, a]: order unchanged
   }
   return false;
 }
 
 // projectTriangleOrigin (:571-611). A = s2, B = s1, C = s0.
-template <class V>
-HFB_HD bool project_triangle(GjkStateT<V>& g) {
+template <bool DEFER, class V>
+HFB_HD bool project_triangle(GjkStateT<V>& g, RayOf& r) {
   const v3 A = g.s2.w, B = g.s1.w, C = g.s0.w;
   const v3 AB = B - A, AC = C - A, ABC = cross(AB, AC);
   int region;
@@ -172,17 +206,15 @@ HFB_HD bool project_triangle(GjkStateT<V>& g) {
     }
   }
   switch (region) {
-    case RG_AC:  // next = [c, a]
-      g.ray = ray_segment(A, C, AC, t);
+    case RG_AC:
+    case RG_AB: {  // AC: next = [c, a]; AB: next = [b, a]
+      const bool ac = region == RG_AC;
+      ray_of_segment<DEFER>(g, r, A, ac ? C : B, t);
+      if (!ac) g.s0 = g.s1;
       g.s1 = g.s2;
       g.rank = 2;
       return false;
-    case RG_AB:  // next = [b, a]
-      g.ray = ray_segment(A, B, AB, t);
-      g.s0 = g.s1;
-      g.s1 = g.s2;
-      g.rank = 2;
-      return false;
+    }
     case RG_A:
       g.ray = A;
       g.s0 = g.s2;
@@ -199,15 +231,15 @@ HFB_HD bool project_triangle(GjkStateT<V>& g) {
         g.s0 = g.s1;
         g.s1 = tmp;
       }
-      g.ray = ray_triangle(ABC, dAO);
+      ray_of_triangle<DEFER>(g, r, ABC, dAO);
       return false;
     }
   }
 }
 
 // projectTetrahedraOrigin (:613-1010). A = s3, B = s2, C = s1, D = s0.
-template <class V>
-HFB_HD bool project_tetra(GjkStateT<V>& g) {
+template <bool DEFER, class V>
+HFB_HD bool project_tetra(GjkStateT<V>& g, RayOf& r) {
   const v3 A = g.s3.w, B = g.s2.w, C = g.s1.w, D = g.s0.w;
   const double aa = sqn(A);
   const double da = dot(D, A), db = dot(D, B), dc = dot(D, C), dd = dot(D, D);
@@ -285,7 +317,7 @@ HFB_HD bool project_tetra(GjkStateT<V>& g) {
     const bool isB = region == RG_AB, isC = region == RG_AC;
     const v3 X = isB ? B : (isC ? C : D);
     const double t = isB ? -ba_aa : (isC ? -ca_aa : -da_aa);
-    g.ray = ray_segment(A, X, X - A, t);
+    ray_of_segment<DEFER>(g, r, A, X, t);
     const V sx = isB ? g.s2 : (isC ? g.s1 : g.s0);
     g.s0 = sx;
     g.s1 = g.s3;
@@ -316,7 +348,7 @@ HFB_HD bool project_tetra(GjkStateT<V>& g) {
     g.s0 = sx;
     g.s1 = sy;
   }
-  g.ray = ray_triangle(N, dAO);
+  ray_of_triangle<DEFER>(g, r, N, dAO);
   return false;
 }
 
@@ -414,8 +446,10 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
   L.w = st.append(g, nv);
   g.rank += 1;
 
-  // check B (:288-293)
-  const double omega = dot(L.dir, L.w) / nrm(L.dir);
+  // check B (:288-293).  Without momentum L.dir is g.ray, and L.rl already holds nrm(g.ray), the same operation on the
+  // same value: gjk_begin sets it with the ray, the end of every step that goes on recomputes it, and the passes'
+  // load_running restores it with the ray.
+  const double omega = dot(L.dir, L.w) / (MOMENTUM ? nrm(L.dir) : L.rl);
   if (omega > st.upper_bound(L, P)) {
     g.distance = omega - st.ssr(L);
     g.status = HFB_GJK_NO_COLLISION_EARLY_STOPPED;
@@ -447,15 +481,21 @@ HFB_HD bool gjk_step(const ShapeD& sa, const ShapeD& sb, const MinkD& md, const 
 
   // simplex sub-solve (:330-350)
   bool inside;
+  RayOf r;
+  r.kind = RAY_SET;
   if (g.rank == 1) {
     g.ray = L.w;
     inside = false;
   } else if (g.rank == 2) {
-    inside = project_line(g);
+    inside = project_line<!MOMENTUM>(g, r);
   } else if (g.rank == 3) {
-    inside = project_triangle(g);
+    inside = project_triangle<!MOMENTUM>(g, r);
   } else {
-    inside = project_tetra(g);
+    inside = project_tetra<!MOMENTUM>(g, r);
+  }
+  if constexpr (!MOMENTUM) {
+    if (r.kind == RAY_SEGMENT) g.ray = ray_segment(r.A, r.X, r.X - r.A, r.t);
+    else if (r.kind == RAY_TRIANGLE) g.ray = ray_triangle(r.A, r.t);
   }
   L.rl = nrm(g.ray);
   if (inside || L.rl == 0) {

@@ -42,10 +42,11 @@ constexpr int pass_blocks_per_sm(bool first, bool momentum) {
 // lanes of a warp touch consecutive doubles (24 KB per block).  gjk_step appends a support point in the lowest slot no
 // live vertex uses: at most 3 vertices are live when it appends, so one is always free.
 // Next to them, what a pair reads but never writes while it iterates: the two radii (finishing reads them) and, with
-// POSE, the relative pose oR1 / ot1 of its Minkowski difference and the parameters p0..p2 of both shapes (the support
-// calls read them), laid out [row][thread] (2 or 20 KB per block).  Without POSE (the passes that run 3 blocks per
-// SM) the support calls read the pose and the parameters from registers.
-enum { RADII_ROWS = 2, POSE_ROWS = 20 };  // ssr0, ssr1; then oR1 row-major (9), ot1 (3), p0..p2 of each shape
+// POSE, the relative pose oR1 / ot1 of its Minkowski difference, the parameters p0..p2 of both shapes (the support
+// calls read them) and the early-stop bound (check B reads it), laid out [row][thread] (2 or 21 KB per block).
+// Without POSE (the passes that run 3 blocks per SM) the support calls read the pose and the parameters, and check B
+// the bound, from registers.
+enum { RADII_ROWS = 2, POSE_ROWS = 21 };  // ssr0, ssr1; then oR1 row-major (9), ot1 (3), p0..p2 of each shape, bound
 template <bool POSE>
 struct SlotStore {
   using V = SVSlot;
@@ -54,12 +55,14 @@ struct SlotStore {
   double* col;   // this thread's column: component c of slot j at col[(6 * j + c) * PASS_THREADS]
   double* pose;  // this thread's column of the `rows` rows: row c at pose[c * PASS_THREADS]
 
-  __device__ __forceinline__ void set_pose(const GjkSetup& S) const {
+  // L: the loop state gjk_begin or load_running set up for the pair (its upper_bound)
+  __device__ __forceinline__ void set_pose(const GjkSetup& S, const GjkLoop& L) const {
     const MinkD& md = S.md;
     const double v[POSE_ROWS] = {md.ssr0,     md.ssr1,     md.oR1.r0.x, md.oR1.r0.y, md.oR1.r0.z,
                                  md.oR1.r1.x, md.oR1.r1.y, md.oR1.r1.z, md.oR1.r2.x, md.oR1.r2.y,
                                  md.oR1.r2.z, md.ot1.x,    md.ot1.y,    md.ot1.z,    S.a.p0,
-                                 S.a.p1,      S.a.p2,      S.b.p0,      S.b.p1,      S.b.p2};
+                                 S.a.p1,      S.a.p2,      S.b.p0,      S.b.p1,      S.b.p2,
+                                 L.upper_bound};
 #pragma unroll
     for (int c = 0; c < rows; ++c) pose[c * PASS_THREADS] = v[c];
   }
@@ -78,14 +81,14 @@ struct SlotStore {
     return R;
   }
   __device__ __forceinline__ v3 ot1() const { return mk(pr(11), pr(12), pr(13)); }
-  // what gjk_begin puts in L.ssr and L.upper_bound, with POSE computed again (same operations) rather than kept in
-  // registers
+  // what gjk_begin puts in L.ssr and L.upper_bound, with POSE read from the rows rather than kept in registers (the
+  // sum of the radii, which only a pair's last step reads, computed again by the same operation)
   __device__ __forceinline__ double ssr(const GjkLoop& L) const {
     if constexpr (POSE) return ssr0() + ssr1();
     else return L.ssr;
   }
-  __device__ __forceinline__ double upper_bound(const GjkLoop& L, const GjkParams& P) const {
-    if constexpr (POSE) return P.distance_upper_bound + ssr(L);
+  __device__ __forceinline__ double upper_bound(const GjkLoop& L, const GjkParams&) const {
+    if constexpr (POSE) return pr(20);
     else return L.upper_bound;
   }
   __device__ __forceinline__ ShapeD shape_at(const ShapeD& s, int c) const {
@@ -311,7 +314,7 @@ __global__ void __launch_bounds__(PASS_THREADS, pass_blocks_per_sm(true, MOM))
         GjkSetup S;
         PairOut o;
         pair_gjk_begin<CAP_PRIM>(in, a.P, S, L, g, o);
-        ss.set_pose(S);
+        ss.set_pose(S, L);
         more = true;
         for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM, Store, MOM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
         fin = !more;
@@ -348,8 +351,8 @@ __global__ void __launch_bounds__(PASS_THREADS, pass_blocks_per_sm(false, MOM))
       const PairIn in = load_pair_in<CAP_PRIM>(a, i);
       GjkSetup S;
       make_setup<CAP_PRIM>(in, S);
-      ss.set_pose(S);
       load_running<MOM>(p.rin, p.st.stride, q, S.md, a.P.gjk, g, L, ss);
+      ss.set_pose(S, L);
       more = true;
       for (int s = 0; s < p.steps && more; ++s) more = gjk_step<1, CAP_PRIM, Store, MOM>(S.a, S.b, S.md, a.P.gjk, g, L, ss);
     }
