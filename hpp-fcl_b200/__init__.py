@@ -11,11 +11,12 @@ from ._pod import *  # noqa: F401,F403
 from .build import build_extension, library_path  # noqa: F401
 from .engine import (  # noqa: F401
     Engine, EngineError, broadphase_config_distance_pairs, broadphase_config_pairs, broadphase_cross_pairs,
-    broadphase_pairs, broadphase_sweep_pairs, build_bvh_obbrss, load_library,
+    broadphase_pairs, broadphase_sweep_pairs, build_bvh_obbrss, load_library, robot_desc,
 )
 from .api import (  # noqa: F401
     BVHModelOBB, BVHModelOBBRSS, Box, Capsule, CollisionRequest, CollisionResult, Cone, Contact, Convex, Cylinder,
     DistanceRequest, DistanceResult, Ellipsoid, Halfspace, Plane, Sphere, Transform3f, TriangleP,
     collide, distance, ComputeCollision, ComputeDistance, BatchQuery,
     AABB, CollisionObject, CollisionCallBackCollect, DynamicAABBTreeCollisionManager, ResidentEnvironment,
+    RobotModel, RobotSamples,
 )

@@ -186,6 +186,19 @@ class CertifyOut(C.Structure):  # hfb_certify_out: per motion its first collidin
                 ("n_uncertified", C.c_void_p)]
 
 
+JOINT_REVOLUTE, JOINT_PRISMATIC = 0, 1  # HFB_JOINT_*
+
+
+class RobotDesc(C.Structure):  # hfb_robot_desc: a kinematic tree of 1-DoF joints and the links on it
+    _fields_ = [("num_joints", C.c_uint32), ("parent", C.c_void_p), ("type", C.c_void_p), ("axis", C.c_void_p),
+                ("placement", C.c_void_p), ("num_links", C.c_uint32), ("link_joint", C.c_void_p),
+                ("link_placement", C.c_void_p), ("link_handles", C.c_void_p)]
+
+
+class RobotSamplesOut(C.Structure):  # hfb_robot_samples_out: the samples' poses and handles, joint values, sweep bounds
+    _fields_ = [("tfs", C.c_void_p), ("handles", C.c_void_p), ("q", C.c_void_p), ("sweep", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

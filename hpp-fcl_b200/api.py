@@ -863,6 +863,94 @@ class ResidentEnvironment:
             pass
 
 
+class RobotSamples:
+    """Link poses of configurations from a RobotModel, in the form ResidentEnvironment's configuration and motion
+    queries take a robot manager: object g * L + i is link i of configuration g.  tfs, handles: the objects; q: the
+    configurations' joint values (n_configs x J) when asked; sweep: the sweep bounds certify_motions() takes, when
+    asked; offsets: the motion offsets of sample_motions(), None for poses()."""
+    _stale = False
+
+    def __init__(self, tfs, handles, q=None, sweep=None, offsets=None):
+        self._tfs, self._handles = tfs, handles
+        self.q, self.sweep, self.offsets = q, sweep, offsets
+
+    @property
+    def tfs(self):
+        return self._tfs
+
+    @property
+    def handles(self):
+        return self._handles
+
+    def size(self):
+        return len(self._handles)
+
+
+class RobotModel:
+    """A kinematic tree of 1-DoF joints with a geometry per link, kept on the device (hfb_robot): Pinocchio's
+    forwardKinematics + updateGeometryPlacements, batched.  joints: (parent, type, axis, placement) per joint, parent -1
+    or an earlier joint, type JOINT_REVOLUTE or JOINT_PRISMATIC, placement a Transform3f (the joint frame in its
+    parent's at q = 0); links: (joint, placement, geometry) per link, joint -1 for fixed to the world.  nq = the number
+    of joints.  include/hppfcl_b200.h states the semantics and the sweep bounds.  close() (or leaving a `with` block)
+    frees it."""
+
+    def __init__(self, joints, links, device=0):
+        self.scene = default_engine(device)
+        self.engine = self.scene.engine
+        parent = [j[0] for j in joints]
+        types = [j[1] for j in joints]
+        axis = np.array([j[2] for j in joints], dtype=np.float64).reshape(-1, 3)
+        placement = _tf_array([j[3] for j in joints]) if joints else np.zeros(0, dtype=P.transform_dtype)
+        link_joint = [l[0] for l in links]
+        link_placement = _tf_array([l[1] for l in links]) if links else np.zeros(0, dtype=P.transform_dtype)
+        self._geoms = [l[2] for l in links]
+        handles = np.array([self.scene.handle(g) for g in self._geoms], dtype=np.uint32)
+        self.scene.commit()
+        self.nq, self.num_links = len(joints), len(links)
+        self._robot = self.engine.robot_create(parent, types, axis, placement, link_joint, link_placement, handles)
+
+    def _sync(self):
+        """the links' geometry changed in place since: its records updated and committed, as a manager's setup() does"""
+        for g in self._geoms:
+            self.scene.handle(g)
+        self.scene.commit()
+
+    def poses(self, q):
+        """q: (n_configs, nq) -> RobotSamples with the links' poses of every configuration"""
+        self._sync()
+        q = np.ascontiguousarray(q, dtype=np.float64).reshape(-1, self.nq)
+        tfs, h = self.engine.robot_poses(self._robot, q)
+        return RobotSamples(tfs, h, q=q)
+
+    def sample_motions(self, q_from, q_to, offsets, sweep=True):
+        """motion m from q_from[m] to q_to[m] ((n_motions, nq) each), offsets[m+1] - offsets[m] samples linear in q,
+        end points included -> RobotSamples with the samples' poses, their q and (sweep=True) the sweep bounds"""
+        self._sync()
+        off = np.asarray(offsets, dtype=np.int64).reshape(-1)
+        if off.shape[0] == 0 or off[0] != 0 or (np.diff(off) < 0).any() or (np.diff(off) > 0x7fffffff).any():
+            raise ValueError("motion offsets must start at 0, not decrease, and hold motions of at most INT32_MAX samples")
+        tfs, h, q, sw = self.engine.robot_sample_motions(self._robot, q_from, q_to, off.astype(np.uint32), q=True,
+                                                         sweep=sweep)
+        return RobotSamples(tfs, h, q=q, sweep=sw, offsets=off.astype(np.uint32))
+
+    def close(self):
+        if getattr(self, "_robot", None) is not None and getattr(self.engine, "h", None):
+            self.engine.robot_destroy(self._robot)
+        self._robot = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _unsupported(o1, o2, what, request=None):
     """the exception the reference throws for this pair (the record carries HFB_PATH_UNSUPPORTED)"""
     mesh = [o for o in (o1, o2) if o.node_type in _MESH_TYPES]

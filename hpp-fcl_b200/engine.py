@@ -84,6 +84,12 @@ def load_library(path=None):
     L.hfb_env_certify_motions.argtypes = [vp, vp, sz, vp, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp]
     L.hfb_env_certify_motions_device.argtypes = [vp, vp, sz, vp, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, vp]
     L.hfb_broadphase_sweep_pairs.argtypes = [sz, vp, vp, sz, sz, vp, sz, vp, sz, sz, vp, vp, sz, vp]
+    L.hfb_robot_create.argtypes = [vp, vp, C.POINTER(vp)]
+    L.hfb_robot_destroy.argtypes = [vp, vp]
+    L.hfb_robot_poses.argtypes = [vp, vp, sz, vp, vp, vp]
+    L.hfb_robot_poses_device.argtypes = [vp, vp, sz, vp, vp, vp, vp]
+    L.hfb_robot_sample_motions.argtypes = [vp, vp, sz, vp, vp, vp, vp]
+    L.hfb_robot_sample_motions_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -252,6 +258,25 @@ def _offsets(offsets):
     if off.dtype.kind not in "ui" or (off.dtype.kind == "i" and (off < 0).any()) or (off > 0xFFFFFFFF).any():
         raise ValueError("motion offsets: integers in [0, 2^32)")
     return np.ascontiguousarray(off, dtype=np.uint32)
+
+
+def robot_desc(parent, types, axis, placement, link_joint, link_placement, link_handles):
+    """an hfb_robot_desc over contiguous copies of the arrays -> (desc, the arrays it points into: keep them alive)"""
+    par = np.ascontiguousarray(parent, dtype=np.int32).reshape(-1)
+    typ = np.ascontiguousarray(types, dtype=np.uint32).reshape(-1)
+    ax = np.ascontiguousarray(axis, dtype=np.float64).reshape(-1, 3)
+    pl = np.ascontiguousarray(placement, dtype=P.transform_dtype).reshape(-1)
+    lj = np.ascontiguousarray(link_joint, dtype=np.int32).reshape(-1)
+    lp = np.ascontiguousarray(link_placement, dtype=P.transform_dtype).reshape(-1)
+    lh = np.ascontiguousarray(link_handles, dtype=np.uint32).reshape(-1)
+    J, L = par.shape[0], lj.shape[0]
+    if typ.shape[0] != J or ax.shape[0] != J or pl.shape[0] != J:
+        raise ValueError("robot model: one type, axis and placement per joint")
+    if lp.shape[0] != L or lh.shape[0] != L:
+        raise ValueError("robot model: one placement and geometry handle per link")
+    keep = (par, typ, ax, pl, lj, lp, lh)
+    desc = P.RobotDesc(J, *[a.ctypes.data for a in keep[:4]], L, *[a.ctypes.data for a in keep[4:]])
+    return desc, keep
 
 
 def _ptr(a):
@@ -740,6 +765,75 @@ class Engine:
                                                           n_motions, _ptr(off), first_motion,
                                                           n_motions - first_motion if num_motions is None else num_motions,
                                                           C.byref(req), C.byref(out), _ptr(stream)))
+
+    # -- robot models (hfb_robot_*) -------------------------------------------------------------------------------
+    def robot_create(self, parent, types, axis, placement, link_joint, link_placement, link_handles):
+        """a robot model on the device (hfb_robot_create): joints (parent: -1 or an earlier joint; types:
+        JOINT_REVOLUTE / JOINT_PRISMATIC; axis: 3 per joint; placement: hfb_transform per joint) and links (link_joint:
+        -1 or a joint; link_placement; committed geometry handles) -> the robot"""
+        desc, keep = robot_desc(parent, types, axis, placement, link_joint, link_placement, link_handles)
+        r = C.c_void_p()
+        self._check(self.L.hfb_robot_create(self.h, C.byref(desc), C.byref(r)))
+        if not hasattr(self, "_robots"):
+            self._robots = {}
+        self._robots[r.value] = (desc.num_joints, desc.num_links)
+        return r
+
+    def robot_destroy(self, robot):
+        self._check(self.L.hfb_robot_destroy(self.h, robot))
+        self._robots.pop(robot.value, None)
+
+    def robot_dims(self, robot):
+        """(num_joints, num_links) of a robot of this engine"""
+        return self._robots[robot.value]
+
+    def robot_poses(self, robot, q, handles=True):
+        """hfb_robot_poses: q (n_configs x J) -> (link poses, n_configs * L; the link handles tiled, or None)"""
+        J, L = self.robot_dims(robot)
+        qa = np.ascontiguousarray(q, dtype=np.float64).reshape(-1)
+        if qa.shape[0] % J:
+            raise ValueError("q: num_joints values per configuration")
+        n = qa.shape[0] // J
+        tfs = np.empty(n * L, dtype=P.transform_dtype)
+        h = np.empty(n * L, dtype=np.uint32) if handles else None
+        self._check(self.L.hfb_robot_poses(self.h, robot, n, _ptr(qa), _ptr(tfs), _ptr(h)))
+        return tfs, h
+
+    def robot_poses_device(self, robot, n_configs, d_q, d_tfs, d_handles=None, stream=0):
+        """hfb_robot_poses_device: q, the poses and the handles are device pointers, ordered on `stream`"""
+        self._check(self.L.hfb_robot_poses_device(self.h, robot, int(n_configs), _ptr(d_q), _ptr(d_tfs), _ptr(d_handles),
+                                                  _ptr(stream)))
+
+    def robot_sample_motions(self, robot, q_from, q_to, offsets, q=False, sweep=True):
+        """hfb_robot_sample_motions: motion m from q_from[m] to q_to[m] (n_motions x J each), sampled
+        offsets[m+1] - offsets[m] times, linear in q -> (poses and handles, n_configs * L; the samples' q, n_configs x J,
+        or None; the sweep bounds, n_configs * L, or None)"""
+        J, L = self.robot_dims(robot)
+        off = _offsets(offsets)
+        n_motions = off.shape[0] - 1
+        qf = np.ascontiguousarray(q_from, dtype=np.float64).reshape(-1)
+        qt = np.ascontiguousarray(q_to, dtype=np.float64).reshape(-1)
+        if qf.shape[0] != n_motions * J or qt.shape[0] != n_motions * J:
+            raise ValueError("q_from, q_to: num_joints values per motion")
+        n = int(off[-1])
+        tfs = np.empty(n * L, dtype=P.transform_dtype)
+        h = np.empty(n * L, dtype=np.uint32)
+        qo = np.empty((n, J)) if q else None
+        sw = np.empty(n * L) if sweep else None
+        out = P.RobotSamplesOut(tfs.ctypes.data, h.ctypes.data, None if qo is None else qo.ctypes.data,
+                                None if sw is None else sw.ctypes.data)
+        self._check(self.L.hfb_robot_sample_motions(self.h, robot, n_motions, _ptr(qf), _ptr(qt), _ptr(off),
+                                                    C.byref(out)))
+        return tfs, h, qo, sw
+
+    def robot_sample_motions_device(self, robot, offsets, d_q_from, d_q_to, d_tfs, d_handles, d_q=None, d_sweep=None,
+                                    stream=0):
+        """hfb_robot_sample_motions_device: the end points and every output are device pointers, ordered on `stream`;
+        the offsets are a host array"""
+        off = _offsets(offsets)
+        out = P.RobotSamplesOut(d_tfs, d_handles, d_q, d_sweep)
+        self._check(self.L.hfb_robot_sample_motions_device(self.h, robot, off.shape[0] - 1, _ptr(d_q_from), _ptr(d_q_to),
+                                                           _ptr(off), C.byref(out), _ptr(stream)))
 
     @staticmethod
     def _objects(handles, tfs):

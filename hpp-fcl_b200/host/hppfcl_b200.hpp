@@ -820,6 +820,7 @@ class DynamicAABBTreeCollisionManager {
 
  private:
   friend class ResidentEnvironment;
+  friend class RobotModel;
   void cross_pairs(const double* boxes_b, size_t n_b, std::vector<uint32_t>& first, std::vector<uint32_t>& second) {
     size_t cap = std::max<size_t>(16 * (objs.size() + n_b), 1024), cnt = 0;
     for (;;) {
@@ -855,6 +856,139 @@ class DynamicAABBTreeCollisionManager {
   std::vector<hfb_transform> tfs;
   std::vector<double> boxes;
   bool stale = true;
+};
+
+/// Link poses of configurations from a RobotModel, in the form ResidentEnvironment's configuration and motion calls
+/// take a robot manager: object g * L + i is link i of configuration g (its table: handles(), transforms()).  It holds
+/// no CollisionObject, so the manager's object calls are not offered on it.  q(): the configurations' joint values
+/// (n_configs x nq); sweep(): the bounds certify_motions takes (sample_motions with sweep = true, else empty);
+/// offsets(): the motion offsets of sample_motions (empty for poses).
+class RobotSamples : public DynamicAABBTreeCollisionManager {
+ public:
+  explicit RobotSamples(int device = 0) : DynamicAABBTreeCollisionManager(device) {}
+  size_t size() const { return handles().size(); }
+  const std::vector<double>& q() const { return q_; }
+  const std::vector<double>& sweep() const { return sweep_; }
+  const std::vector<uint32_t>& offsets() const { return offsets_; }
+  template <class... A> void registerObject(A&&...) = delete;
+  template <class... A> void registerObjects(A&&...) = delete;
+  template <class... A> void unregisterObject(A&&...) = delete;
+  template <class... A> void clear(A&&...) = delete;
+  template <class... A> void setup(A&&...) = delete;
+  template <class... A> void update(A&&...) = delete;
+  template <class... A> void collide(A&&...) = delete;
+  template <class... A> void pairs(A&&...) = delete;
+  template <class... A> void getObjects(A&&...) = delete;
+
+ private:
+  friend class RobotModel;
+  std::vector<double> q_, sweep_;
+  std::vector<uint32_t> offsets_;
+};
+
+/// A kinematic tree of 1-DoF joints with a geometry per link, kept on the device (hfb_robot): Pinocchio's
+/// forwardKinematics + updateGeometryPlacements, batched.  Joint: parent (-1 or an earlier joint), type
+/// (HFB_JOINT_REVOLUTE / HFB_JOINT_PRISMATIC), axis, placement (the joint frame in its parent's at q = 0); Link: joint
+/// (-1 for fixed to the world), placement, geometry.  nq = the number of joints.  include/hppfcl_b200.h states the
+/// semantics and the sweep bounds.  A malformed model, q of the wrong size or malformed offsets throw
+/// std::invalid_argument.  Owns the hfb_robot.
+class RobotModel {
+ public:
+  struct Joint {
+    int32_t parent;
+    uint32_t type;
+    Vec3f axis;
+    Transform3f placement;
+  };
+  struct Link {
+    int32_t joint;
+    Transform3f placement;
+    CollisionGeometryPtr_t geometry;
+  };
+  RobotModel(const std::vector<Joint>& joints, const std::vector<Link>& links, int device = 0)
+      : device(device), C(Context::instance(device)) {
+    if (joints.size() > 64 || links.size() > 0xffffffffull) throw std::invalid_argument("robot model: too many joints or links");
+    std::vector<int32_t> parent, link_joint;
+    std::vector<uint32_t> type, handles;
+    std::vector<double> axis;
+    std::vector<hfb_transform> placement, link_placement;
+    for (const Joint& j : joints) {
+      parent.push_back(j.parent);
+      type.push_back(j.type);
+      for (int k = 0; k < 3; ++k) axis.push_back(j.axis[k]);
+      placement.push_back(j.placement.pod());
+    }
+    for (const Link& l : links) {
+      link_joint.push_back(l.joint);
+      link_placement.push_back(l.placement.pod());
+      geoms.push_back(l.geometry);
+      handles.push_back(C.handle(l.geometry.get()));
+    }
+    C.commit();
+    hfb_robot_desc d{(uint32_t)joints.size(), parent.data(), type.data(),       axis.data(),  placement.data(),
+                     (uint32_t)links.size(),  link_joint.data(), link_placement.data(), handles.data()};
+    C.check(hfb_robot_create(C.raw(), &d, &robot));
+    nq_ = joints.size();
+    L = links.size();
+  }
+  ~RobotModel() {
+    if (robot) hfb_robot_destroy(C.raw(), robot);
+  }
+  RobotModel(const RobotModel&) = delete;
+  RobotModel& operator=(const RobotModel&) = delete;
+  size_t nq() const { return nq_; }
+  size_t num_links() const { return L; }
+
+  /// q: n_configs x nq joint values -> the links' poses of every configuration (hfb_robot_poses)
+  RobotSamples poses(const std::vector<double>& q) {
+    if (q.size() % nq_) throw std::invalid_argument("q: nq values per configuration");
+    const size_t n = q.size() / nq_;
+    sync();
+    RobotSamples s(device);
+    s.hs.resize(n * L);
+    s.tfs.resize(n * L);
+    C.check(hfb_robot_poses(C.raw(), robot, n, q.data(), s.tfs.data(), s.hs.data()));
+    s.stale = false;
+    s.q_ = q;
+    return s;
+  }
+
+  /// motion m from q_from[m] to q_to[m] (n_motions x nq each), offsets[m+1] - offsets[m] samples linear in q, end points
+  /// included -> the samples' poses, their q and (sweep = true) the sweep bounds (hfb_robot_sample_motions)
+  RobotSamples sample_motions(const std::vector<double>& q_from, const std::vector<double>& q_to,
+                              const std::vector<uint32_t>& offsets, bool sweep = true) {
+    if (offsets.empty() || offsets[0] != 0) throw std::invalid_argument("motion offsets must start at 0");
+    for (size_t m = 0; m + 1 < offsets.size(); ++m) {
+      if (offsets[m + 1] < offsets[m]) throw std::invalid_argument("motion offsets decrease");
+      if (offsets[m + 1] - offsets[m] > 0x7fffffffu) throw std::invalid_argument("a motion has more than INT32_MAX samples");
+    }
+    const size_t n_motions = offsets.size() - 1, n = offsets.back();
+    if (q_from.size() != n_motions * nq_ || q_to.size() != n_motions * nq_)
+      throw std::invalid_argument("q_from, q_to: nq values per motion");
+    sync();
+    RobotSamples s(device);
+    s.hs.resize(n * L);
+    s.tfs.resize(n * L);
+    s.q_.resize(n * nq_);
+    if (sweep) s.sweep_.resize(n * L);
+    hfb_robot_samples_out o{s.tfs.data(), s.hs.data(), s.q_.data(), sweep ? s.sweep_.data() : nullptr};
+    C.check(hfb_robot_sample_motions(C.raw(), robot, n_motions, q_from.data(), q_to.data(), offsets.data(), &o));
+    s.stale = false;
+    s.offsets_ = offsets;
+    return s;
+  }
+
+ private:
+  // the links' geometry changed in place since: its records updated and committed, as a manager's setup() does
+  void sync() {
+    for (const CollisionGeometryPtr_t& g : geoms) C.handle(g.get());
+    C.commit();
+  }
+  int device;
+  Context& C;
+  std::vector<CollisionGeometryPtr_t> geoms;
+  hfb_robot* robot = nullptr;
+  size_t nq_ = 0, L = 0;
 };
 
 /// config 5 in one call: the manager's candidate pairs through the batched narrow phase.  Returns, per candidate

@@ -444,3 +444,38 @@ def chain_self_pairs(n_links, skip=2):
     and are not checked, as an SRDF disables adjacent links) -> (P, 2) uint32; 105 pairs for 16 links"""
     i, j = np.triu_indices(n_links, k=skip)
     return np.stack([i, j], axis=1).astype(np.uint32)
+
+
+def chain_robot_model(w):
+    """robot_motions' (or robot_vs_environment's) chain as a robot model, in the arrays hfb_robot_desc takes: prismatic
+    joints x and y carry the base (joints 0 and 1, on the world), then the yaw joint (about z, at the base) and the
+    bending joints, about z (link k even) or y (k odd), each placed link_len along its parent's z axis; link k hangs on
+    joint k + 2 at link_len / 2 along its z axis.  The q layout is [x, y, q_0 .. q_{L-1}].
+    -> dict: parent, types, axis, placement (J = L + 2 joints), link_joint, link_placement, geom (the geometry slot of
+    each link, as w["geom_a"] and w["register"] number them); with w from robot_motions also q (the samples' joint
+    values, n_configs x J, the base read back from link 0's pose) and q_from / q_to (each motion's first and last
+    sample, n_motions x J)."""
+    L, ll = w["n_links"], w["link_len"]
+    J = L + 2
+    parent = np.arange(-1, J - 1, dtype=np.int32)
+    types = np.array([P.JOINT_PRISMATIC] * 2 + [P.JOINT_REVOLUTE] * L, dtype=np.uint32)
+    axis = np.zeros((J, 3))
+    axis[0, 0] = axis[1, 1] = 1.0
+    axis[2 + np.arange(L), np.where(np.arange(L) % 2 == 0, 2, 1)] = 1.0
+    placement = identity_transforms(J)
+    placement["T"][3:, 2] = ll
+    link_placement = identity_transforms(L)
+    link_placement["T"][:, 2] = 0.5 * ll
+    out = dict(parent=parent, types=types, axis=axis, placement=placement, link_joint=np.arange(2, J, dtype=np.int32),
+               link_placement=link_placement, geom=np.asarray(w["geom_a"][:L]))
+    if "q" in w:
+        tf0 = w["tf_a"][::L]  # link 0 of every sample: its start is the base
+        base = tf0["T"] - 0.5 * ll * tf0["R"].reshape(-1, 3, 3)[:, 2, :]  # (R is column-major: row 2 is the z axis)
+        q = np.concatenate([base[:, :2], w["q"]], axis=1)
+        off = np.asarray(w["offsets"], dtype=np.int64)
+        first = off[:-1]
+        q_from = q[np.minimum(first, len(q) - 1)]
+        q_to = q[np.maximum(off[1:] - 1, 0)]
+        q_to[:, :2] = q_from[:, :2]  # (the base stays put along a motion)
+        out.update(q=q, q_from=np.ascontiguousarray(q_from), q_to=np.ascontiguousarray(q_to))
+    return out

@@ -764,6 +764,91 @@ int hfb_broadphase_sweep_pairs(size_t n_a, const double* aabbs, const double* sw
                                const uint32_t* motion_offsets, size_t first_motion, size_t num_motions, uint32_t* first,
                                uint32_t* second, size_t capacity, size_t* n_pairs);
 
+/* ---- a robot model on the device: forward kinematics, motion sampling and sweep bounds ---------------------------
+ * What Pinocchio's forwardKinematics(model, data, q) followed by updateGeometryPlacements(model, data, geom_model,
+ * geom_data) computes for a kinematic tree of 1-DoF joints, batched over configurations, with the results laid out as
+ * the hfb_env_* calls above take set A: object g*L + i is link i of configuration g, so a planner chains these calls
+ * with the env queries on one stream and uploads joint values instead of poses.
+ * The model (hfb_robot_desc, validated on the host; a malformed one is HFB_ERR_INVALID_ARGUMENT and nothing is
+ * created):
+ *   num_joints J, 1..64, with nq = J: configuration g is q[g*J .. g*J + J).  Per joint j: parent[j] -1 (the world) or
+ *   < j, so the joints come in topological order; type[j] HFB_JOINT_REVOLUTE or HFB_JOINT_PRISMATIC; axis[3j..3j+3),
+ *   normalised at create (a zero or non-finite axis is refused); placement[j], the joint frame in its parent's frame at
+ *   q = 0.  num_links L >= 1, with L * J <= UINT32_MAX.  Per link i: link_joint[i], -1 for fixed to the world or a joint index;
+ *   link_placement[i]; link_handles[i], a committed geometry handle.  Null arrays are refused.
+ * Semantics:
+ *   joint frame   M_j = M_parent(j) o placement_j o X_j(q_j), M_parent = identity for a joint on the world; X_j is the
+ *                 rotation by q_j about the unit axis (Rodrigues) for a revolute joint, the translation by q_j * axis
+ *                 for a prismatic one;
+ *   link pose     M_link_joint(i) o link_placement_i; link_placement_i for a link fixed to the world.
+ *   sin and cos come from the library's own fdlibm restatement (csrc/hfb_kin.cuh), below 1 ulp for |q| <= 2^20 * pi/2
+ *   (about 1.647e6 rad) and NaN beyond, so the device and a host build of the same code give the same bits.  A
+ *   non-finite q is not an error: it propagates to NaN poses, which the narrow phase's rules for non-finite input handle.
+ * The geometry: after a later hfb_geom_commit the handles are checked again (in range, not released) and the local
+ * boxes the sweep bounds use are read again; after hfb_geom_clear every call on the robot is refused until it is
+ * destroyed -- the rules of hfb_env.  hfb_ctx_destroy frees the robots a context still owns.
+ * Counts: n_configs * L <= UINT32_MAX, as the env calls' n_a.
+ *   hfb_robot_poses: n_configs x J joint values -> tfs (n_configs * L link poses) and, when handles is not null, the
+ *     link handles tiled n_configs times.
+ *   hfb_robot_sample_motions: motion m goes from q_from[m*J ..] to q_to[m*J ..]; motion_offsets (n_motions + 1 uint32,
+ *     HOST memory in both forms) are checked as hfb_env_collide_motions checks them, n_configs = offsets[n_motions].
+ *     Sample k of an n-sample motion, configuration offsets[m] + k, is q_from at k = 0, exactly q_to at k = n - 1 and
+ *     q_from + (k / (n - 1)) * (q_to - q_from) in between: OMPL's RealVectorStateSpace::interpolate, linear in q.  A
+ *     one-sample motion is q_from; an empty motion is allowed.  Outputs (hfb_robot_samples_out): tfs and handles as
+ *     hfb_robot_poses writes them; q (may be null): the samples' joint values, n_configs x J; sweep (may be null): the
+ *     bounds hfb_env_certify_motions takes.
+ * Sweep bounds.  sweep[g*L + i] bounds the path length of every point of link i over the segment from sample g to g+1:
+ *     s = sum over the joints k on the path from the root to link i of |q_{g+1,k} - q_{g,k}| * rho_k, with rho_k = 1 for
+ *     a prismatic k and, for a revolute k, rho_k = the sum over the joints j strictly below k on that path of
+ *     |translation(placement_j)|, plus max(|q_{g,j}|, |q_{g+1,j}|) for the prismatic ones among them, plus
+ *     |translation(link_placement_i)| + r_i, where r_i is the largest corner norm of the geometry's committed local box
+ *     (+inf for an unbounded geometry; a joint that does not move adds 0).  The argument: a point moves at the speed
+ *     sum_k |dq_k/dt| * (its distance to k's axis) for revolute k, plus |dq_k/dt| for prismatic k.  k's axis passes
+ *     through the origin of M_k, and the point's distance to that origin is at most rho_k by the triangle inequality
+ *     down the path (a revolute joint does not move its own origin, a prismatic j moves it by |q_j|).  q is linear over
+ *     the segment, so |q_j| is largest at an end point and the integral of |dq_k/dt| is |q_{g+1,k} - q_{g,k}|.  s is
+ *     computed in round-to-nearest, then multiplied by 1 + J * 2^-46, far above the sum's rounding error, and rounded to
+ *     the next double, so the host and the device give the same bits.  The entry at a motion's last sample is 0, as
+ *     are those of links fixed to the world and of segments where no joint of the path moves.
+ * Refusals: a null context, robot or array, malformed offsets, or a count past the 32-bit rule is
+ * HFB_ERR_INVALID_ARGUMENT, and nothing is written.
+ *   hfb_robot_poses / hfb_robot_sample_motions: HOST buffers, blocking.
+ *   *_device: q (q_from, q_to) and every output in DEVICE memory, ordered on `cuda_stream`; the call does not block
+ *     (the offsets are read on the host).  It orders itself after the context's previous *_device call as those do.
+ * One kernel serves both: one thread per (configuration, link), walking the link's path from the root; every frame is
+ * evaluated by the one formula above, so no result depends on scheduling. */
+#define HFB_JOINT_REVOLUTE 0u
+#define HFB_JOINT_PRISMATIC 1u
+typedef struct hfb_robot_desc {
+  uint32_t num_joints;
+  const int32_t* parent;
+  const uint32_t* type;
+  const double* axis;
+  const hfb_transform* placement;
+  uint32_t num_links;
+  const int32_t* link_joint;
+  const hfb_transform* link_placement;
+  const uint32_t* link_handles;
+} hfb_robot_desc;
+typedef struct hfb_robot hfb_robot;
+typedef struct hfb_robot_samples_out {
+  hfb_transform* tfs; /* n_configs * L */
+  uint32_t* handles;  /* n_configs * L */
+  double* q;          /* n_configs * J, may be null */
+  double* sweep;      /* n_configs * L, may be null */
+} hfb_robot_samples_out;
+int hfb_robot_create(hfb_ctx* ctx, const hfb_robot_desc* desc, hfb_robot** out);
+int hfb_robot_destroy(hfb_ctx* ctx, hfb_robot* robot);
+int hfb_robot_poses(hfb_ctx* ctx, hfb_robot* robot, size_t n_configs, const double* q, hfb_transform* tfs,
+                    uint32_t* handles);
+int hfb_robot_poses_device(hfb_ctx* ctx, hfb_robot* robot, size_t n_configs, const double* d_q, hfb_transform* d_tfs,
+                           uint32_t* d_handles, void* cuda_stream);
+int hfb_robot_sample_motions(hfb_ctx* ctx, hfb_robot* robot, size_t n_motions, const double* q_from, const double* q_to,
+                             const uint32_t* motion_offsets, const hfb_robot_samples_out* out);
+int hfb_robot_sample_motions_device(hfb_ctx* ctx, hfb_robot* robot, size_t n_motions, const double* d_q_from,
+                                    const double* d_q_to, const uint32_t* motion_offsets,
+                                    const hfb_robot_samples_out* d_out, void* cuda_stream);
+
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
  * 58-61, distance.h:53-56) take their geometry and pose from the objects.  A scene here is a table of objects
