@@ -436,6 +436,25 @@ inline const char* config_template_error(size_t links, size_t n_pairs, const uin
   if (std::adjacent_find(keys.begin(), keys.end()) != keys.end()) return "self-pair template: a pair listed twice";
   return nullptr;
 }
+// a set A of n_a objects as configurations of `links` objects each, the range [g0, g0 + ng) of them and the template of
+// n_tpl self pairs; null when they meet the conditions
+inline const char* config_range_error(size_t n_a, size_t links, size_t g0, size_t ng, size_t n_tpl, const uint32_t* tpl) {
+  if (links == 0 || n_a % links) return "n_a is not a multiple of links_per_config";
+  if (g0 > n_a / links || ng > n_a / links - g0) return "configuration range past the end";
+  if (n_tpl > 0xffffffffull) return "self-pair template too large";
+  return config_template_error(links, n_tpl, tpl);
+}
+// the n_motions + 1 offsets of n_motions runs of configurations: from 0 on, not decreasing, at most INT32_MAX samples
+// per motion; null when they meet these.  That off[n_motions] is the number of configurations is the caller's check.
+inline const char* motion_offsets_error(size_t n_motions, const uint32_t* off) {
+  if (n_motions > 0xffffffffull) return "too many motions";
+  if (off[0] != 0) return "motion offsets do not start at 0";
+  for (size_t m = 0; m < n_motions; ++m) {
+    if (off[m + 1] < off[m]) return "motion offsets decrease";
+    if (off[m + 1] - off[m] > 0x7fffffffu) return "a motion has more than INT32_MAX samples";
+  }
+  return nullptr;
+}
 // self pair t of the configurations from g0 on: configuration g0 + t / P, template entry t % P -> (*a, *b), object
 // indices in A; true when both objects have a box and the boxes overlap (AABB::overlap, closed intervals)
 HFB_HD bool config_pair(const double* bb, uint32_t links, const uint32_t* tpl, uint32_t n_pairs, uint32_t g0, size_t t,
