@@ -199,6 +199,17 @@ class RobotSamplesOut(C.Structure):  # hfb_robot_samples_out: the samples' poses
     _fields_ = [("tfs", C.c_void_p), ("handles", C.c_void_p), ("q", C.c_void_p), ("sweep", C.c_void_p)]
 
 
+class ValidateParams(C.Structure):  # hfb_validate_params: the initial and the largest depth, the samples per round
+    _fields_ = [("initial_depth", C.c_uint32), ("max_depth", C.c_uint32), ("max_samples", C.c_uint64)]
+
+
+class ValidateOut(C.Structure):  # hfb_validate_out: per motion its status, certified prefix, first collision and witness
+    _fields_ = [("status", C.c_void_p), ("t_valid", C.c_void_p), ("t_collide", C.c_void_p), ("kind", C.c_void_p),
+                ("first", C.c_void_p), ("second", C.c_void_p), ("contacts", C.c_void_p), ("n_rounds", C.c_void_p),
+                ("n_samples", C.c_void_p), ("n_env_candidates", C.c_void_p), ("n_self_candidates", C.c_void_p),
+                ("n_unsupported", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("pairs_processed", C.c_uint64),
                 ("epa_pairs", C.c_uint64), ("bv_tests", C.c_uint64), ("leaf_tests", C.c_uint64),

@@ -803,6 +803,36 @@ class ResidentEnvironment:
         return self.engine.env_certify_motions(self._env, h, t, sw, links_per_config, tpl, off, req, first_motion,
                                                num_motions)[:3]
 
+    def validate_motions(self, robot_model, q_from, q_to, self_pairs, *, initial_depth, max_depth, max_samples,
+                         request=None, first_motion=0, num_motions=None):
+        """A planner's progressive motion validation: motion m runs from q_from[m] to q_to[m] ((n_motions, nq) each)
+        of the RobotModel, linear in q.  Each motion is cut into 2^initial_depth segments, certified as
+        certify_motions() certifies them, and the uncertified segments are split again, down to 2^-max_depth of the
+        motion, with at most max_samples samples per round (include/hppfcl_b200.h, hfb_env_validate_motions, states
+        the rounds and their guarantee).  -> MotionValidation: per motion status (0 valid, 1 collides, 2 unresolved, -1
+        outside the range), t_valid (the certified prefix is [0, t_valid]), t_collide (the earliest colliding sample
+        found, -1 for none), the witness there (kind, first, second: link indices, or an environment index for kind 0;
+        contacts), and the counts n_rounds, n_samples, n_env_candidates, n_self_candidates, n_unsupported."""
+        request = request or CollisionRequest()
+        if request.num_max_contacts == 0 and request.security_margin != -np.inf:
+            raise ValueError("Invalid number of max contacts (current value is 0).")
+        d0, d, cap = int(initial_depth), int(max_depth), int(max_samples)
+        if d0 < 0 or d0 > d or d > 30 or cap < 2:
+            raise ValueError("need 0 <= initial_depth <= max_depth <= 30 and max_samples >= 2")
+        qf = np.asarray(q_from, dtype=np.float64)
+        qt = np.asarray(q_to, dtype=np.float64)
+        if qf.ndim != 2 or qf.shape[1] != robot_model.nq or qt.shape != qf.shape:
+            raise ValueError("q_from, q_to: (n_motions, nq) each")
+        n = qf.shape[0]
+        num_motions = n - first_motion if num_motions is None else num_motions
+        if first_motion < 0 or num_motions < 0 or first_motion + num_motions > n:
+            raise ValueError("motion range past the end")
+        tpl = self._template_args(robot_model.num_links, self_pairs)
+        robot_model._sync()
+        r = self.engine.env_validate_motions(self._env, robot_model._robot, qf, qt, tpl, d0, d, cap, request._pod,
+                                             int(first_motion), int(num_motions))
+        return MotionValidation(**r)
+
     @staticmethod
     def _motion_args(n_objects, links_per_config, motion_offsets, first_motion, num_motions):
         """the offsets and the motion range as the C ABI takes them; ones the C ABI refuses raise ValueError (the C++
@@ -861,6 +891,15 @@ class ResidentEnvironment:
             self.close()
         except Exception:
             pass
+
+
+class MotionValidation:
+    """What ResidentEnvironment.validate_motions() returns: per motion status, t_valid, t_collide and the witness
+    (kind, first, second, contacts), arrays of n_motions; the counts n_rounds, n_samples, n_env_candidates,
+    n_self_candidates, n_unsupported, ints."""
+
+    def __init__(self, **fields):
+        self.__dict__.update(fields)
 
 
 class RobotSamples:

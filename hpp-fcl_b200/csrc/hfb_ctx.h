@@ -155,6 +155,9 @@ struct hfb_ctx {
   DevBuf sc_moff, sc_mot;   // hfb_env_collide_motions: the motion offsets, the per-motion state (hfb::BpMotions)
   DevBuf sc_sweep, sc_side, sc_cpass;  // hfb_env_certify_motions: the sweep bounds (host form), the sides and widened
                                       // boxes of A, the per-sample pass flags (hfb::BpCertify)
+  // hfb_env_validate_motions: the per-motion state and staged outputs, the open segments (two lists: this round's and
+  // the next), the per-segment scans, the round's samples and runs, its counters, and CUB's scratch
+  DevBuf sc_vmot, sc_vseg[2], sc_vscan, sc_vsmp, sc_vrun, sc_vcnt, sc_vcub;
   // resident environments: every hfb_geom_commit / hfb_geom_clear is counted, so that an env notices them
   std::vector<hfb_env*> envs;
   std::vector<hfb_robot*> robots;  // robot models (hfb_robot_create), checked against the same counters
@@ -188,6 +191,11 @@ struct hfb_robot {
   DevBuf off, q_in, tfs, handles, q_out, sweep;
   uint64_t commits = 0, clears = 0;  // the context's counters when the handles were last checked
 };
+
+// hfb_robot.cu: a robot of this context whose geometry is still valid (as env_ready; the links' reach is read again
+// after a commit), and the robot's model arguments for a launch on stream s (links whose reach changed uploaded first)
+int robot_ready(hfb_ctx* ctx, hfb_robot* r);
+int robot_model_args(hfb_ctx* ctx, hfb_robot* r, cudaStream_t s, hfb::KinAtArgs* a);
 
 inline int fail(hfb_ctx* c, int code, const std::string& msg) {
   if (c) c->err = msg;

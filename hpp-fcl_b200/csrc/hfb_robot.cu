@@ -59,7 +59,38 @@ __global__ void __launch_bounds__(256) k_robot(const KinArgs a) {
   }
 }
 
+// hfb_env_validate_motions' samples: one thread per (sample, link) as k_robot, at the sample's dyadic position
+__global__ void __launch_bounds__(256) k_robot_at(const KinAtArgs a) {
+  const size_t n = a.n_samples * a.L;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+    const uint32_t g = (uint32_t)(t / a.L), i = (uint32_t)(t % a.L);
+    const KinLink link = a.links[i];
+    const uint32_t J = a.J, m = __ldg(a.m + g), k = __ldg(a.k + g);
+    const double* from = a.q_from + (size_t)m * J;
+    const double* to = a.q_to + (size_t)m * J;
+    auto q0 = [&](uint32_t j) { return kin_sample(__ldg(from + j), __ldg(to + j), k, a.n_pos); };
+    hfb_transform tf;
+    kin_link_pose(a.joints, link, a.path_list, q0, tf);
+    if (a.sweep) {
+      auto q1 = [&](uint32_t j) { return kin_sample(__ldg(from + j), __ldg(to + j), k + a.len, a.n_pos); };
+      a.sweep[t] = __ldg(a.seg + g) ? kin_link_sweep(a.joints, link, a.path_list, J, q0, q1) : 0.0;
+    }
+    a.tfs[t] = tf;
+    a.handles[t] = link.handle;
+  }
+}
+
 }  // namespace
+
+int robot_at_launch(const KinAtArgs& a, int num_sms, cudaStream_t s) {
+  const size_t n = a.n_samples * a.L;
+  if (n == 0) return cudaSuccess;
+  const size_t cap = (size_t)(num_sms > 0 ? num_sms : 1) * 8;
+  const unsigned blocks = (unsigned)((n + 255) / 256 < cap ? (n + 255) / 256 : cap);
+  k_robot_at<<<blocks, 256, 0, s>>>(a);
+  return (int)cudaGetLastError();
+}
 
 int robot_launch(const KinArgs& a, bool sample, int num_sms, cudaStream_t s) {
   const size_t n = a.n_configs * a.L;
@@ -100,6 +131,8 @@ void robot_reach(hfb_ctx* ctx, hfb_robot* r) {
   for (hfb::KinLink& k : r->links) k.reach = hfb::kin_link_reach(k, ctx->local_aabbs.data() + 6 * (size_t)k.handle);
 }
 
+}  // namespace
+
 // a robot of this context whose geometry is still valid: as env_ready, plus the links' reach read again after a commit
 int robot_ready(hfb_ctx* ctx, hfb_robot* r) {
   if (std::find(ctx->robots.begin(), ctx->robots.end(), r) == ctx->robots.end())
@@ -119,6 +152,22 @@ int robot_ready(hfb_ctx* ctx, hfb_robot* r) {
   }
   return HFB_OK;
 }
+
+int robot_model_args(hfb_ctx* ctx, hfb_robot* r, cudaStream_t s, hfb::KinAtArgs* a) {
+  if (r->links_stale) {
+    CK(cudaMemcpyAsync(static_cast<char*>(r->model.p) + r->links_at, r->links.data(), r->L * sizeof(hfb::KinLink),
+                       cudaMemcpyHostToDevice, s));
+    r->links_stale = false;
+  }
+  a->joints = static_cast<const hfb::KinJoint*>(r->model.p);
+  a->links = reinterpret_cast<const hfb::KinLink*>(static_cast<char*>(r->model.p) + r->links_at);
+  a->path_list = static_cast<const uint8_t*>(r->model.p) + r->path_at;
+  a->J = r->J;
+  a->L = r->L;
+  return HFB_OK;
+}
+
+namespace {
 
 // hfb_robot_poses and hfb_robot_sample_motions in both forms.  Sampling when `off` is not null: q and q_to are the
 // motions' end points, n_configs = off[n_motions].  Host form (dev == false): every pointer is host memory, the call

@@ -31,4 +31,28 @@ struct KinArgs {
 // returns a cudaError_t as int
 int robot_launch(const KinArgs& a, bool sample, int num_sms, cudaStream_t s);
 
+// One launch of k_robot_at (hfb_env_validate_motions): n_samples samples at dyadic positions of their motions.  Sample
+// t is motion m[t] (q_from / q_to: its end points, J values per motion) at position k[t] of n_pos = 2^D + 1 (kin_sample's
+// formula, so the depth-d samples are those of 2^d + 1 evenly spaced ones); its L link poses and handles go to
+// tfs / handles[t * L ..].  When seg[t] is set, sweep[t * L ..] gets the links' sweep bounds over [k[t], k[t] + len];
+// else 0 (a run's last sample).  sweep may be null.
+struct KinAtArgs {
+  const KinJoint* joints;
+  const KinLink* links;
+  const uint8_t* path_list;
+  uint32_t J, L;
+  size_t n_samples;
+  const double* q_from;
+  const double* q_to;
+  const uint32_t* m;
+  const uint32_t* k;
+  const uint8_t* seg;
+  uint32_t n_pos, len;
+  hfb_transform* tfs;
+  uint32_t* handles;
+  double* sweep;
+};
+// returns a cudaError_t as int
+int robot_at_launch(const KinAtArgs& a, int num_sms, cudaStream_t s);
+
 }  // namespace hfb

@@ -13,9 +13,12 @@
 #include <utility>
 #include <vector>
 
+#include <cub/device/device_scan.cuh>
+
 #include "hfb_ctx.h"
 #include "hfb_broadphase.cuh"
 #include "hfb_broadphase.h"
+#include "hfb_validate.cuh"
 
 // hfb_scene_collide: the colliding pairs of a scene -- object indices and contact record -- appended in no
 // particular order
@@ -66,6 +69,187 @@ __global__ void __launch_bounds__(256) k_flag_configs(const hfb_contact* r, cons
     if (me) atomicAdd(counts, (unsigned)__popc(me));
     if (ms) atomicAdd(counts + 1, (unsigned)__popc(ms));
   }
+}
+
+// ---- hfb_env_validate_motions: the bookkeeping between rounds (the rules: hfb_validate.cuh) --------------------------
+// A round's open segments, sorted by (motion, start): w, the motion's index in the range, and the start position.  The
+// per-segment passes run over `bound` entries, a host-side bound on the list's length *n (the device holds it): entries
+// past it get 0 in every scanned array.  Per motion w of the range: c (earliest colliding sample), f (start of the
+// earliest stuck segment), u (start of the earliest segment closed without a certificate); kValNone for none.
+struct ValSegs {
+  uint32_t* w;
+  uint32_t* a;
+};
+struct ValMotions {
+  uint32_t *c, *f, *u;
+};
+// round 0: the admitted prefix of the range's 2^d0 segments per motion (val_round0), and each motion's state
+__global__ void __launch_bounds__(256) k_val_init(ValSegs sg, size_t n_seg, size_t n_range, uint64_t n_full, uint32_t partial,
+                                                  uint32_t per, uint32_t len, ValMotions st, uint32_t* d_n) {
+  const size_t n = n_seg > n_range ? n_seg : n_range;
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (size_t)gridDim.x * blockDim.x) {
+    if (t < n_seg) {
+      sg.w[t] = (uint32_t)(t / per);
+      sg.a[t] = (uint32_t)(t % per) * len;
+    }
+    if (t < n_range) {
+      const uint32_t adm = val_round0_admitted(t, n_full, partial, per);
+      st.c[t] = kValNone;
+      st.f[t] = st.u[t] = adm < per ? adm * len : kValNone;
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *d_n = (uint32_t)n_seg;
+}
+// per segment: its cost and whether it starts a run
+__global__ void __launch_bounds__(256) k_val_cost(ValSegs sg, const uint32_t* d_n, uint32_t bound, uint32_t len,
+                                                  uint32_t* cost, uint32_t* nr) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= bound) return;
+  if (i >= *d_n) {
+    cost[i] = nr[i] = 0;
+    return;
+  }
+  const bool r = val_new_run(i == 0, i ? sg.w[i - 1] : 0, i ? sg.a[i - 1] : 0, sg.w[i], sg.a[i], len);
+  cost[i] = val_cost(r);
+  nr[i] = r;
+}
+// the round's totals from the inclusive scans of the costs and run flags: tot[0] admitted segments, tot[1] samples,
+// tot[2] runs (the last admitted segment writes them; zeros for an empty list)
+__global__ void __launch_bounds__(256) k_val_admit(const uint32_t* d_n, uint32_t bound, const uint32_t* cscan,
+                                                   const uint32_t* rscan, uint32_t cap, uint32_t* tot) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, n = *d_n;
+  if (i == 0 && n == 0) tot[0] = tot[1] = tot[2] = 0;
+  if (i >= bound || i >= n || !val_admitted(cscan[i], cap)) return;
+  if (i + 1 == n || !val_admitted(cscan[i + 1], cap)) {
+    tot[0] = i + 1;
+    tot[1] = cscan[i];
+    tot[2] = rscan[i];
+  }
+}
+// the round's samples (motion, position, whether a segment starts there) and the runs' offsets into them, from the
+// n_adm admitted segments
+__global__ void __launch_bounds__(256) k_val_samples(ValSegs sg, uint32_t n_adm, uint32_t len, const uint32_t* cscan,
+                                                     const uint32_t* nr, const uint32_t* rscan, uint32_t* sw, uint32_t* sk,
+                                                     uint8_t* sseg, uint32_t* off) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_adm) return;
+  const uint32_t g = val_start_sample(cscan[i]), w = sg.w[i], a = sg.a[i];
+  sw[g] = w;
+  sk[g] = a;
+  sseg[g] = 1;
+  if (nr[i]) off[rscan[i] - 1] = g;
+  if (i + 1 == n_adm || nr[i + 1]) {  // the run ends here: its last sample
+    sw[g + 1] = w;
+    sk[g + 1] = a + len;
+    sseg[g + 1] = 0;
+  }
+  if (i + 1 == n_adm) off[rscan[i]] = cscan[i];
+}
+// each run's first colliding sample (certify's first_invalid) into its motion's c
+__global__ void __launch_bounds__(256) k_val_collide(uint32_t n_runs, const int32_t* fi, const uint32_t* off,
+                                                     const uint32_t* sw, const uint32_t* sk, ValMotions st) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_runs || fi[r] < 0) return;
+  const uint32_t g = off[r] + (uint32_t)fi[r];
+  atomicMin(st.c + sw[g], sk[g]);
+}
+// the segment rules: kids[i] = 2 for a split segment, else 0; a stuck or dropped segment's start into its motion's u,
+// a stuck one's into f.  Thread 0 adds the round's unsupported records (*n_unsup) to *acc.
+__global__ void __launch_bounds__(256) k_val_rules(ValSegs sg, const uint32_t* d_n, uint32_t bound, uint32_t n_adm,
+                                                   bool deepest, uint32_t L, const uint32_t* cscan, const uint8_t* cert,
+                                                   const double* sweep, ValMotions st, uint32_t* kids,
+                                                   const unsigned* n_unsup, unsigned long long* acc) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) *acc += *n_unsup;
+  if (i >= bound) return;
+  if (i >= *d_n) {
+    kids[i] = 0;
+    return;
+  }
+  const uint32_t w = sg.w[i], a = sg.a[i];
+  const bool admitted = i < n_adm;
+  bool certified = false, finite = true;
+  if (admitted) {
+    const uint32_t g = val_start_sample(cscan[i]);
+    certified = cert[g];
+    for (uint32_t l = 0; l < L; ++l) finite = finite && sweep[(size_t)g * L + l] <= DBL_MAX;  // (NaN, +inf: not)
+  }
+  const ValRule rule = val_rule(admitted, certified, a, st.c[w], deepest, finite);
+  if (rule == VAL_DROPPED || rule == VAL_STUCK) atomicMin(st.u + w, a);
+  if (rule == VAL_STUCK) atomicMin(st.f + w, a);
+  kids[i] = rule == VAL_SPLIT ? 2u : 0u;
+}
+// the frontier: of a split segment, the halves that start before its motion's f
+__global__ void __launch_bounds__(256) k_val_keep(ValSegs sg, const uint32_t* d_n, uint32_t half, ValMotions st,
+                                                  uint32_t* kids) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= *d_n || !kids[i]) return;
+  const uint32_t f = st.f[sg.w[i]], a = sg.a[i];
+  kids[i] = (uint32_t)val_keep(a, f) + (uint32_t)val_keep(a + half, f);
+}
+// the next round's list from the exclusive scan of kids, in (motion, start) order, and its length *d_n_next
+__global__ void __launch_bounds__(256) k_val_compact(ValSegs sg, const uint32_t* d_n, uint32_t half, ValMotions st,
+                                                     const uint32_t* kids, const uint32_t* kscan, ValSegs nx,
+                                                     uint32_t* d_n_next) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, n = *d_n;
+  if (i >= n) return;
+  if (i + 1 == n) *d_n_next = kscan[i] + kids[i];
+  if (!kids[i]) return;
+  const uint32_t w = sg.w[i], a = sg.a[i], f = st.f[w];
+  uint32_t p = kscan[i];
+  for (uint32_t b : {a, a + half}) {
+    if (!val_keep(b, f)) continue;
+    nx.w[p] = w;
+    nx.a[p] = b;
+    ++p;
+  }
+}
+// the outputs of hfb_env_validate_motions (each array n_motions long): the range's motions from their state
+// (val_result), the others -1, 0, -1; wflag[w] = 1 for the range's colliding motions
+struct ValOut {
+  int8_t* status;
+  double* t_valid;
+  double* t_collide;
+};
+__global__ void __launch_bounds__(256) k_val_final(uint32_t n_motions, uint32_t m0, uint32_t n_range, uint32_t D,
+                                                   ValMotions st, ValOut o, uint32_t* wflag) {
+  const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n_motions) return;
+  if (m < m0 || m - m0 >= n_range) {
+    o.status[m] = -1;
+    o.t_valid[m] = 0.0;
+    o.t_collide[m] = -1.0;
+    return;
+  }
+  const uint32_t w = m - m0;
+  val_result(st.c[w], st.u[w], D, o.status + m, o.t_valid + m, o.t_collide + m);
+  if (wflag) wflag[w] = st.c[w] != kValNone;
+}
+// the witness samples: the range's colliding motions, in order (widx: the exclusive scan of wflag), each at its c
+__global__ void __launch_bounds__(256) k_val_wsamples(uint32_t n_range, const uint32_t* wflag, const uint32_t* widx,
+                                                      ValMotions st, uint32_t* sw, uint32_t* sk, uint8_t* sseg,
+                                                      uint32_t* n_w) {
+  const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w >= n_range) return;
+  if (w + 1 == n_range) *n_w = widx[w] + wflag[w];
+  if (!wflag[w]) return;
+  const uint32_t p = widx[w];
+  sw[p] = w;
+  sk[p] = st.c[w];
+  sseg[p] = 0;
+}
+// the witnesses of the one-sample motions (hfb_env_collide_motions' outputs over the witness samples) to their
+// motions: A indices p * L + i back to link indices
+__global__ void __launch_bounds__(256) k_val_witness(uint32_t n_w, uint32_t m0, uint32_t L, const uint32_t* sw,
+                                                     const int8_t* kind, const uint32_t* first, const uint32_t* second,
+                                                     const hfb_contact* rec, BpMotions o) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_w || kind[p] < 0) return;
+  const uint32_t m = m0 + sw[p], base = p * L;
+  if (o.kind) o.kind[m] = kind[p];
+  if (o.first) o.first[m] = first[p] - base;
+  if (o.second) o.second[m] = kind[p] == 0 ? second[p] : second[p] - base;
+  if (o.rec) o.rec[m] = rec[p];
 }
 
 extern "C" {
@@ -1082,6 +1266,46 @@ struct EnvCollideMotions {
 // hfb_env_certify_motions' outputs, checked before the context is looked at
 static bool certify_ok(const hfb_certify_out* o) { return o && (o->first_invalid || o->first_uncertified || o->certified); }
 
+// The certification that hfb_env_certify_motions and hfb_env_validate_motions share, with A in the env's table and the
+// template in ctx->sc_tpl: the sides of A's objects of the configurations [t.g0, t.g0 + t.ng) from the device sweep
+// bounds d_sweep and their widened boxes (c.sides, the boxes after the 2 * n_a sides), the candidates of the widened
+// boxes and of sweep_pair with their collide() records (configs_candidates; *cand and *split as it gives them), then
+// bp_certify_launch into c's flags, state and outputs, counting in ctx->sc_cnt[1] (unsupported) and [2] (uncertified).
+// c holds the motions (device offsets, [m0, m1)), the configurations (g0, ng), the sides and the pass flags.
+static int certify_body(hfb_ctx* ctx, hfb_env* e, size_t n_a, const ConfigTpl& t, const hfb_collision_request* req,
+                        bool minus_inf, const BpCertify& c, const double* d_sweep, cudaStream_t s, unsigned* cand,
+                        unsigned* split) {
+  const size_t links = t.links;
+  double* d_wbb = c.sides + 2 * n_a;
+  const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
+  const size_t a_lo = t.g0 * links, a_hi = (t.g0 + t.ng) * links;
+  bool sided = false;  // (the finder runs twice when the candidate lists grow; the sides are made once)
+  if (int rc = configs_candidates(
+          ctx, e, n_a, t, req, minus_inf, nullptr, s, cand, split,
+          [&](const double* d_bb, const double** d_qb, int* nl) {
+            *d_qb = d_wbb;
+            if (sided) return 0;
+            sided = true;
+            return bp_sweep_sides_launch(d_bb, d_sweep, a_lo, a_hi, c, d_wbb, s, nl);
+          },
+          [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
+            return bp_sweep_pairs_launch(d_bb, c, d_tpl, t.n, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
+          }))
+    return rc;
+  unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
+  CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
+  // under minus_inf no record exists (collision.cpp:73-76): every pair passes, every sample is valid
+  const size_t n_recs = minus_inf ? 0 : *cand;
+  int nl = 0;
+  if (bp_certify_launch(static_cast<const hfb_contact*>(ctx->sc_out.p), static_cast<const uint32_t*>(ctx->sc_pf.p),
+                        static_cast<const uint32_t*>(ctx->sc_ps.p), n_recs, *split, (uint32_t)n_a,
+                        static_cast<const double*>(ctx->sc_bb.p), static_cast<const double*>(e->bb.p), c, d_cnt + 1, s,
+                        &nl) != 0)
+    return fail(ctx, HFB_ERR_CUDA, "k_cert_pairs launch failed");
+  ctx->stats.kernel_launches += (uint64_t)nl;
+  return HFB_OK;
+}
+
 // hfb_env_certify_motions (the template in ctx->sc_tpl, the offsets in ctx->sc_moff, the sweep bounds in
 // ctx->sc_sweep in the host form): the sides of the range's A objects and their widened boxes (ctx->sc_side), the
 // candidates of the widened boxes and of sweep_pair with their collide() records (configs_candidates), then the
@@ -1142,7 +1366,6 @@ struct EnvCertifyMotions {
     c.g0 = (unsigned)t.g0;
     c.ng = (unsigned)t.ng;
     c.sides = static_cast<double*>(ctx->sc_side.p);
-    double* d_wbb = c.sides + 2 * n_a;
     c.pass = static_cast<uint8_t*>(ctx->sc_cpass.p);
     if (o.dev) {
       c.first_invalid = out->first_invalid;
@@ -1156,35 +1379,11 @@ struct EnvCertifyMotions {
         c.certified = static_cast<uint8_t*>(ctx->sc_flags.p);
       }
     }
-    const uint32_t* d_tpl = static_cast<const uint32_t*>(ctx->sc_tpl.p);
-    const size_t a_lo = t.g0 * links, a_hi = (t.g0 + t.ng) * links;
-    bool sided = false;  // (the finder runs twice when the candidate lists grow; the sides are made once)
     unsigned cand = 0, split = 0;
-    if (int rc = configs_candidates(
-            ctx, e, n_a, t, req, minus_inf, nullptr, s, &cand, &split,
-            [&](const double* d_bb, const double** d_qb, int* nl) {
-              *d_qb = d_wbb;
-              if (sided) return 0;
-              sided = true;
-              return bp_sweep_sides_launch(d_bb, d_sweep, a_lo, a_hi, c, d_wbb, s, nl);
-            },
-            [&](const double* d_bb, uint32_t* pf, uint32_t* ps, size_t cap, unsigned* d_cnt, int* nl) {
-              return bp_sweep_pairs_launch(d_bb, c, d_tpl, t.n, pf, ps, cap, d_cnt, ctx->num_sms, s, nl);
-            }))
-      return rc;
+    if (int rc = certify_body(ctx, e, n_a, t, req, minus_inf, c, d_sweep, s, &cand, &split)) return rc;
     CK(o.count(out->n_env_candidates, split));
     CK(o.count(out->n_self_candidates, cand - split));
     unsigned* d_cnt = static_cast<unsigned*>(ctx->sc_cnt.p);
-    CK(cudaMemsetAsync(d_cnt + 1, 0, 2 * sizeof(unsigned), s));
-    // under minus_inf no record exists (collision.cpp:73-76): every pair passes, every sample is valid
-    const size_t n_recs = minus_inf ? 0 : cand;
-    int nl = 0;
-    if (bp_certify_launch(static_cast<const hfb_contact*>(ctx->sc_out.p), static_cast<const uint32_t*>(ctx->sc_pf.p),
-                          static_cast<const uint32_t*>(ctx->sc_ps.p), n_recs, split, (uint32_t)n_a,
-                          static_cast<const double*>(ctx->sc_bb.p), static_cast<const double*>(e->bb.p), c, d_cnt + 1, s,
-                          &nl) != 0)
-      return fail(ctx, HFB_ERR_CUDA, "k_cert_pairs launch failed");
-    ctx->stats.kernel_launches += (uint64_t)nl;
     if (!o.dev) {
       const size_t m0 = first_motion, nm = num_motions;
       if (out->first_invalid) CK(o.copy(out->first_invalid + m0, c.first_invalid + m0, nm * 4));
@@ -1196,6 +1395,311 @@ struct EnvCertifyMotions {
     CK(o.finish());
     return HFB_OK;
   }
+};
+
+// hfb_env_validate_motions' pure argument checks, before the context is looked at
+static bool validate_ok(size_t n_motions, const double* q_from, const double* q_to, size_t n_self_pairs,
+                        const uint32_t* self_pairs, size_t first_motion, size_t num_motions,
+                        const hfb_collision_request* req, const hfb_validate_params* p, const hfb_validate_out* o) {
+  if (!req || !p || !o || !o->status || !o->t_valid || !o->t_collide || (n_self_pairs && !self_pairs)) return false;
+  if (p->initial_depth > p->max_depth || p->max_depth > 30 || p->max_samples < 2) return false;
+  if (n_motions > 0xffffffffull || first_motion > n_motions || num_motions > n_motions - first_motion) return false;
+  return !(num_motions && (!q_from || !q_to));
+}
+
+// an exclusive (ex) or inclusive scan of n uint32 on stream s, CUB's scratch in ctx->sc_vcub
+static int val_scan(hfb_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n, bool ex, cudaStream_t s) {
+  size_t bytes = 0;
+  CK(ex ? cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, (int)n, s)
+        : cub::DeviceScan::InclusiveSum(nullptr, bytes, in, out, (int)n, s));
+  CK(ctx->sc_vcub.reserve(bytes));
+  CK(ex ? cub::DeviceScan::ExclusiveSum(ctx->sc_vcub.p, bytes, in, out, (int)n, s)
+        : cub::DeviceScan::InclusiveSum(ctx->sc_vcub.p, bytes, in, out, (int)n, s));
+  ctx->stats.kernel_launches++;
+  return HFB_OK;
+}
+
+static unsigned val_blocks(size_t n) { return (unsigned)((n + 255) / 256); }
+
+// hfb_env_validate_motions (include/hppfcl_b200.h states the rounds and their rules): the robot samples each round's
+// runs straight into the env's table (k_robot_at), certify_body certifies them as motions, and the k_val_* kernels
+// apply the rules and build the next round's list.  The call blocks once per round for its totals (the admitted
+// segments, samples and runs that size the launches), where certify_body blocks, and once for the witness count.
+// Buffers: ctx->sc_vmot the per-motion state (and the host form's staged outputs), sc_vseg the two lists, sc_vscan the
+// per-segment scans, sc_vsmp the samples, sc_vrun the runs and the certified flags, sc_sweep the sweep bounds.
+struct EnvValidateMotions {
+  const hfb_collision_request* req;
+  const hfb_validate_out* out;
+  ConfigTpl t;  // links: the robot's L (set by check()); g0 and ng: each round's samples
+  hfb_robot* robot;
+  size_t n_motions;
+  const double* q_from;
+  const double* q_to;
+  size_t first_motion, num_motions;
+  hfb_validate_params p;
+  bool minus_inf = false;
+
+  const ConfigTpl* tpl() const { return &t; }
+  bool witness() const { return out->kind || out->first || out->second || out->contacts; }
+  int check(hfb_ctx* ctx) {
+    if (int rc = collide_prelude(ctx, req, &minus_inf)) return rc;
+    if (int rc = robot_ready(ctx, robot)) return rc;
+    t.links = robot->L;
+    return HFB_OK;
+  }
+  int zero(hfb_ctx* ctx, QueryOut& o, size_t) const {
+    CK(o.zero(out->n_rounds, sizeof(uint32_t)));
+    for (uint64_t* c : {out->n_samples, out->n_env_candidates, out->n_self_candidates, out->n_unsupported})
+      CK(o.zero(c, sizeof(uint64_t)));
+    return HFB_OK;
+  }
+  bool empty(const hfb_env*, size_t) const { return false; }  // (run() writes every motion's outputs)
+  int run(hfb_ctx* ctx, hfb_env* e, size_t, QueryOut& o) const {
+    const cudaStream_t s = o.s;
+    const uint32_t L = (uint32_t)t.links, J = robot->J, D = p.max_depth, d0 = p.initial_depth;
+    const size_t n = n_motions, n_range = num_motions, m0 = first_motion;
+    // the cap: the caller's, at most 2^29 (so that a round's list, at most twice the samples before it, and the scan of
+    // its costs, at most twice its length, stay below 2^31), and within the env calls' 32-bit object count
+    // (samples * L + n_b < 2^32)
+    uint64_t cap64 = p.max_samples < (1ull << 29) ? p.max_samples : (1ull << 29);
+    const uint64_t fit = (0xffffffffull - e->n_b) / L;
+    if (fit < cap64) cap64 = fit;
+    const uint32_t cap = (uint32_t)cap64;
+    hfb::KinAtArgs ka{};
+    if (int rc = robot_model_args(ctx, robot, s, &ka)) return rc;
+    ka.n_pos = (1u << D) + 1u;
+    if (o.dev) {
+      ka.q_from = q_from + m0 * J;
+      ka.q_to = q_to + m0 * J;
+    } else if (n_range) {
+      CK(robot->q_in.reserve(n_range * J * 16));
+      double* d_q = static_cast<double*>(robot->q_in.p);
+      CK(cudaMemcpyAsync(d_q, q_from + m0 * J, n_range * J * 8, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(d_q + n_range * J, q_to + m0 * J, n_range * J * 8, cudaMemcpyHostToDevice, s));
+      ka.q_from = d_q;
+      ka.q_to = d_q + n_range * J;
+    }
+    // per motion: the state, the witness flags and their scan, then (host form) the staged outputs
+    const size_t r4 = up(n_range * 4);
+    CK(ctx->sc_vmot.reserve(5 * r4 + (o.dev ? 0 : up(n) * 2 + up(n * 8) * 2 + up(n * 4) * 2 + up(n * sizeof(hfb_contact)))));
+    char* vm = static_cast<char*>(ctx->sc_vmot.p);
+    const ValMotions st{reinterpret_cast<uint32_t*>(vm), reinterpret_cast<uint32_t*>(vm + r4),
+                        reinterpret_cast<uint32_t*>(vm + 2 * r4)};
+    uint32_t* wflag = reinterpret_cast<uint32_t*>(vm + 3 * r4);
+    uint32_t* widx = reinterpret_cast<uint32_t*>(vm + 4 * r4);
+    ValOut vo{out->status, out->t_valid, out->t_collide};
+    BpMotions wo{};
+    wo.kind = out->kind, wo.first = out->first, wo.second = out->second, wo.rec = out->contacts;
+    if (!o.dev) {
+      char* at = vm + 5 * r4;
+      auto take = [&](size_t bytes) {
+        char* q = at;
+        at += up(bytes);
+        return q;
+      };
+      vo.status = reinterpret_cast<int8_t*>(take(n));
+      vo.t_valid = reinterpret_cast<double*>(take(n * 8));
+      vo.t_collide = reinterpret_cast<double*>(take(n * 8));
+      int8_t* k = reinterpret_cast<int8_t*>(take(n));
+      uint32_t* f = reinterpret_cast<uint32_t*>(take(n * 4));
+      uint32_t* sc = reinterpret_cast<uint32_t*>(take(n * 4));
+      hfb_contact* r = reinterpret_cast<hfb_contact*>(take(n * sizeof(hfb_contact)));
+      if (wo.kind) wo.kind = k;
+      if (wo.first) wo.first = f;
+      if (wo.second) wo.second = sc;
+      if (wo.rec) wo.rec = r;
+    }
+    CK(ctx->sc_vcnt.reserve(64));
+    uint32_t* d_nl = static_cast<uint32_t*>(ctx->sc_vcnt.p);  // the two lists' lengths
+    uint32_t* d_tot = d_nl + 2;                                // a round's totals, the witness count
+    unsigned long long* d_acc = reinterpret_cast<unsigned long long*>(d_nl + 8);  // the unsupported records
+    CK(cudaMemsetAsync(d_acc, 0, 8, s));
+    // round 0
+    const uint32_t per = 1u << d0;
+    uint64_t n_full = 0;
+    uint32_t partial = 0;
+    val_round0(n_range, per, cap, &n_full, &partial);
+    uint64_t bound = n_full * per + partial;  // (<= cap)
+    int cur = 0;
+    CK(ctx->sc_vseg[0].reserve(bound * 8 + 8));
+    if (n_range) {  // (a list of cap / 8 entries: w, then a, as every round reads it)
+      const size_t cb = (size_t)(ctx->sc_vseg[0].cap / 8);
+      const ValSegs sg{static_cast<uint32_t*>(ctx->sc_vseg[0].p), static_cast<uint32_t*>(ctx->sc_vseg[0].p) + cb};
+      const size_t nt = bound > n_range ? bound : n_range;
+      const size_t blocks = val_blocks(nt) < (size_t)ctx->num_sms * 8 ? val_blocks(nt) : (size_t)ctx->num_sms * 8;
+      k_val_init<<<(unsigned)blocks, 256, 0, s>>>(sg, bound, n_range, n_full, partial, per, 1u << (D - d0), st, d_nl);
+      ctx->stats.kernel_launches++;
+    }
+    uint32_t rounds = 0;
+    uint64_t n_samples = 0, n_env = 0, n_self = 0;
+    for (uint32_t depth = d0; n_range && bound && depth <= D; ++depth) {
+      const uint32_t len = 1u << (D - depth), nb = (uint32_t)bound;
+      const size_t cb = (size_t)(ctx->sc_vseg[cur].cap / 8);
+      const ValSegs sg{static_cast<uint32_t*>(ctx->sc_vseg[cur].p), static_cast<uint32_t*>(ctx->sc_vseg[cur].p) + cb};
+      CK(ctx->sc_vscan.reserve((size_t)nb * 24));
+      uint32_t* cost = static_cast<uint32_t*>(ctx->sc_vscan.p);
+      uint32_t *cscan = cost + nb, *nr = cost + 2 * (size_t)nb, *rscan = cost + 3 * (size_t)nb;
+      uint32_t *kids = cost + 4 * (size_t)nb, *kscan = cost + 5 * (size_t)nb;
+      k_val_cost<<<val_blocks(nb), 256, 0, s>>>(sg, d_nl + cur, nb, len, cost, nr);
+      ctx->stats.kernel_launches++;
+      if (int rc = val_scan(ctx, cost, cscan, nb, false, s)) return rc;
+      if (int rc = val_scan(ctx, nr, rscan, nb, false, s)) return rc;
+      k_val_admit<<<val_blocks(nb), 256, 0, s>>>(d_nl + cur, nb, cscan, rscan, cap, d_tot);
+      ctx->stats.kernel_launches++;
+      uint32_t tot[3] = {0, 0, 0};
+      CK(cudaMemcpyAsync(tot, d_tot, sizeof tot, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      const uint32_t n_adm = tot[0], smp = tot[1], runs = tot[2];
+      if (n_adm == 0) break;  // (no open segment left)
+      ++rounds;
+      n_samples += smp;
+      // the samples and runs, the robot's poses and sweeps into the env's table, then the certification of the runs
+      CK(ctx->sc_vsmp.reserve((size_t)smp * 9));
+      uint32_t* sw = static_cast<uint32_t*>(ctx->sc_vsmp.p);
+      uint32_t* sk = sw + smp;
+      uint8_t* sseg = reinterpret_cast<uint8_t*>(sk + smp);
+      CK(ctx->sc_vrun.reserve(up(((size_t)runs + 1) * 4) + up((size_t)runs * 4) + smp));
+      uint32_t* off = static_cast<uint32_t*>(ctx->sc_vrun.p);
+      int32_t* fi = reinterpret_cast<int32_t*>(static_cast<char*>(ctx->sc_vrun.p) + up(((size_t)runs + 1) * 4));
+      uint8_t* cert = reinterpret_cast<uint8_t*>(fi) + up((size_t)runs * 4);
+      k_val_samples<<<val_blocks(n_adm), 256, 0, s>>>(sg, n_adm, len, cscan, nr, rscan, sw, sk, sseg, off);
+      ctx->stats.kernel_launches++;
+      const size_t n_a = (size_t)smp * L;
+      if (int rc = env_make_room(ctx, e, n_a, s)) return rc;
+      CK(ctx->sc_sweep.reserve(n_a * 8));
+      double* d_sweep = static_cast<double*>(ctx->sc_sweep.p);
+      hfb::KinAtArgs a = ka;
+      a.n_samples = smp;
+      a.m = sw;
+      a.k = sk;
+      a.seg = sseg;
+      a.len = len;
+      a.tfs = static_cast<hfb_transform*>(e->tf.p) + (e->head - n_a);
+      a.handles = static_cast<uint32_t*>(e->h.p) + (e->head - n_a);
+      a.sweep = d_sweep;
+      if (int err = hfb::robot_at_launch(a, ctx->num_sms, s))
+        return cuda_fail(ctx, static_cast<cudaError_t>(err), "k_robot_at launch");
+      ctx->stats.kernel_launches++;
+      CK(ctx->sc_side.reserve(n_a * 64));
+      CK(ctx->sc_cpass.reserve((size_t)smp * 2));
+      CK(ctx->sc_mot.reserve(bp_certify_bytes(runs, false)));
+      BpCertify c = bp_certify_carve(ctx->sc_mot.p, runs, false);
+      c.off = off;
+      c.m0 = 0;
+      c.m1 = runs;
+      c.links = L;
+      c.g0 = 0;
+      c.ng = smp;
+      c.sides = static_cast<double*>(ctx->sc_side.p);
+      c.pass = static_cast<uint8_t*>(ctx->sc_cpass.p);
+      c.first_invalid = fi;
+      c.certified = cert;
+      ConfigTpl tr = t;
+      tr.g0 = 0;
+      tr.ng = smp;
+      unsigned cand = 0, split = 0;
+      if (int rc = certify_body(ctx, e, n_a, tr, req, minus_inf, c, d_sweep, s, &cand, &split)) return rc;
+      n_env += split;
+      n_self += cand - split;
+      // the rules, the frontier and the next round's list
+      k_val_collide<<<val_blocks(runs), 256, 0, s>>>(runs, fi, off, sw, sk, st);
+      k_val_rules<<<val_blocks(nb), 256, 0, s>>>(sg, d_nl + cur, nb, n_adm, depth == D, L, cscan, cert, d_sweep, st, kids,
+                                                 static_cast<const unsigned*>(ctx->sc_cnt.p) + 1, d_acc);
+      k_val_keep<<<val_blocks(nb), 256, 0, s>>>(sg, d_nl + cur, len / 2, st, kids);
+      ctx->stats.kernel_launches += 3;
+      if (int rc = val_scan(ctx, kids, kscan, nb, true, s)) return rc;
+      const uint64_t next = 2 * (uint64_t)n_adm;
+      CK(ctx->sc_vseg[1 - cur].reserve(next * 8 + 8));
+      const size_t nc = (size_t)(ctx->sc_vseg[1 - cur].cap / 8);
+      const ValSegs nx{static_cast<uint32_t*>(ctx->sc_vseg[1 - cur].p), static_cast<uint32_t*>(ctx->sc_vseg[1 - cur].p) + nc};
+      k_val_compact<<<val_blocks(nb), 256, 0, s>>>(sg, d_nl + cur, len / 2, st, kids, kscan, nx, d_nl + 1 - cur);
+      ctx->stats.kernel_launches++;
+      cur = 1 - cur;
+      bound = next;
+    }
+    // the outputs, then the witnesses: one hfb_env_collide_motions pass over the colliding motions' samples at c
+    const bool wit = witness() && n_range;
+    if (n) {
+      k_val_final<<<val_blocks(n), 256, 0, s>>>((uint32_t)n, (uint32_t)m0, (uint32_t)n_range, D, st, vo,
+                                                wit ? wflag : nullptr);
+      ctx->stats.kernel_launches++;
+      if (witness()) {
+        int nl = 0;
+        if (bp_motions_init_launch(n, wo, s, &nl) != 0) return fail(ctx, HFB_ERR_CUDA, "k_mot_init launch failed");
+        ctx->stats.kernel_launches += (uint64_t)nl;
+      }
+    }
+    if (wit) {
+      if (int rc = val_scan(ctx, wflag, widx, (uint32_t)n_range, true, s)) return rc;
+      CK(ctx->sc_vsmp.reserve(n_range * 9));
+      uint32_t* sw = static_cast<uint32_t*>(ctx->sc_vsmp.p);
+      uint32_t* sk = sw + n_range;
+      uint8_t* sseg = reinterpret_cast<uint8_t*>(sk + n_range);
+      k_val_wsamples<<<val_blocks(n_range), 256, 0, s>>>((uint32_t)n_range, wflag, widx, st, sw, sk, sseg, d_tot + 3);
+      ctx->stats.kernel_launches++;
+      uint32_t n_w = 0;
+      CK(cudaMemcpyAsync(&n_w, d_tot + 3, 4, cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      if (n_w) {
+        const size_t n_a = (size_t)n_w * L;
+        if (int rc = env_make_room(ctx, e, n_a, s)) return rc;
+        hfb::KinAtArgs a = ka;
+        a.n_samples = n_w;
+        a.m = sw;
+        a.k = sk;
+        a.seg = sseg;
+        a.tfs = static_cast<hfb_transform*>(e->tf.p) + (e->head - n_a);
+        a.handles = static_cast<uint32_t*>(e->h.p) + (e->head - n_a);
+        if (int err = hfb::robot_at_launch(a, ctx->num_sms, s))
+          return cuda_fail(ctx, static_cast<cudaError_t>(err), "k_robot_at launch");
+        ctx->stats.kernel_launches++;
+        CK(ctx->sc_vrun.reserve(up((size_t)n_w) + 2 * up((size_t)n_w * 4) + (size_t)n_w * sizeof(hfb_contact)));
+        char* r = static_cast<char*>(ctx->sc_vrun.p);
+        int8_t* kind = reinterpret_cast<int8_t*>(r);
+        uint32_t* first = reinterpret_cast<uint32_t*>(r + up(n_w));
+        uint32_t* second = reinterpret_cast<uint32_t*>(r + up(n_w) + up((size_t)n_w * 4));
+        hfb_contact* rec = reinterpret_cast<hfb_contact*>(r + up(n_w) + 2 * up((size_t)n_w * 4));
+        const hfb_motions_out mo{nullptr, kind, first, second, rec, nullptr, nullptr, nullptr, nullptr};
+        std::vector<uint32_t> offsets(n_w + 1);
+        for (uint32_t k = 0; k <= n_w; ++k) offsets[k] = k;
+        ConfigTpl tw = t;
+        tw.g0 = 0;
+        tw.ng = n_w;
+        EnvCollideMotions q{req, &mo, tw, n_w, offsets.data(), 0, n_w, minus_inf};
+        QueryOut inner{s, true};
+        if (int rc = q.zero(ctx, inner, n_a)) return rc;
+        if (int rc = q.run(ctx, e, n_a, inner)) return rc;
+        k_val_witness<<<val_blocks(n_w), 256, 0, s>>>(n_w, (uint32_t)m0, L, sw, kind, first, second, rec, wo);
+        ctx->stats.kernel_launches++;
+      }
+    }
+    // the counts: rounds, samples and candidates known here, the unsupported records on the device
+    if (o.dev) {
+      const uint64_t hv[3] = {n_samples, n_env, n_self};
+      uint64_t* dst[3] = {out->n_samples, out->n_env_candidates, out->n_self_candidates};
+      if (out->n_rounds) CK(cudaMemcpyAsync(out->n_rounds, &rounds, 4, cudaMemcpyHostToDevice, s));
+      for (int k = 0; k < 3; ++k)
+        if (dst[k]) CK(cudaMemcpyAsync(dst[k], hv + k, 8, cudaMemcpyHostToDevice, s));
+    } else {
+      CK(o.copy(out->status, vo.status, n));
+      CK(o.copy(out->t_valid, vo.t_valid, n * 8));
+      CK(o.copy(out->t_collide, vo.t_collide, n * 8));
+      CK(o.copy(out->kind, wo.kind, n));
+      CK(o.copy(out->first, wo.first, n * 4));
+      CK(o.copy(out->second, wo.second, n * 4));
+      CK(o.copy(out->contacts, wo.rec, n * sizeof(hfb_contact)));
+    }
+    CK(o.copy(out->n_unsupported, d_acc, 8));
+    CK(o.finish());
+    if (!o.dev) {
+      if (out->n_rounds) *out->n_rounds = rounds;
+      if (out->n_samples) *out->n_samples = n_samples;
+      if (out->n_env_candidates) *out->n_env_candidates = n_env;
+      if (out->n_self_candidates) *out->n_self_candidates = n_self;
+    }
+    return HFB_OK;
+  }
+  static size_t up(size_t b) { return (b + 255) & ~(size_t)255; }
 };
 
 // the arguments of a configurations query beyond the pointers: the layout of A, the configuration range and the template
@@ -1228,6 +1732,7 @@ static int query_args(hfb_ctx* ctx, size_t n_a, Query& q) {
 }
 static int query_args(hfb_ctx* ctx, size_t n_a, EnvCollideMotions& q) { return motions_args(ctx, n_a, q); }
 static int query_args(hfb_ctx* ctx, size_t n_a, EnvCertifyMotions& q) { return motions_args(ctx, n_a, q); }
+// (hfb_env_validate_motions' A is made by the call: only its template, over the robot's links, is the caller's)
 
 // The frame of the hfb_env_* queries (EnvCollide, EnvCollideConfigs, EnvDistance, EnvDistanceConfigs), with their
 // pointers checked: the lock, the query's and the env's checks, A uploaded into the env's table in front of B (and
@@ -1261,8 +1766,10 @@ static int env_call(hfb_ctx* ctx, hfb_env* env, Form form, void* stream, size_t 
   if (int rc = env_make_room(ctx, env, n_a, o.s)) return rc;
   const size_t off = env->head - n_a;
   const cudaMemcpyKind kind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-  CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, h_a, n_a * 4, kind, o.s));
-  CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tf_a, n_a * sizeof(hfb_transform), kind, o.s));
+  if (n_a) {  // (hfb_env_validate_motions makes its A itself)
+    CK(cudaMemcpyAsync(static_cast<uint32_t*>(env->h.p) + off, h_a, n_a * 4, kind, o.s));
+    CK(cudaMemcpyAsync(static_cast<hfb_transform*>(env->tf.p) + off, tf_a, n_a * sizeof(hfb_transform), kind, o.s));
+  }
   if (tpl) {
     CK(ctx->sc_tpl.reserve(tpl->n * 8 + 8));
     if (tpl->n) CK(cudaMemcpyAsync(ctx->sc_tpl.p, tpl->pairs, tpl->n * 8, cudaMemcpyHostToDevice, o.s));
@@ -1445,6 +1952,34 @@ int hfb_env_certify_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
   return env_call(ctx, env, Form::device, stream, n_a, d_handles_a, d_tfs_a,
                   EnvCertifyMotions{req, d_out, {links_per_config, n_self_pairs, self_pairs, 0, 0}, n_motions,
                                     motion_offsets, first_motion, num_motions, d_sweep});
+}
+
+// A planner's progressive motion validation (hfb_validate_out in include/hppfcl_b200.h): each motion sampled by the
+// robot on the device, certified segment by segment, and the uncertified segments split until each motion is proven
+// free, found colliding or at its resolution -- hpp-core's continuous path validation (Dichotomy / Progressive).
+int hfb_env_validate_motions(hfb_ctx* ctx, hfb_env* env, hfb_robot* robot, size_t n_motions, const double* q_from,
+                             const double* q_to, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_motion,
+                             size_t num_motions, const hfb_collision_request* req, const hfb_validate_params* p,
+                             const hfb_validate_out* out) {
+  if (!ctx || !env || !robot ||
+      !validate_ok(n_motions, q_from, q_to, n_self_pairs, self_pairs, first_motion, num_motions, req, p, out))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::host, nullptr, 0, nullptr, nullptr,
+                  EnvValidateMotions{req, out, {0, n_self_pairs, self_pairs, 0, 0}, robot, n_motions, q_from, q_to,
+                                     first_motion, num_motions, *p});
+}
+
+int hfb_env_validate_motions_device(hfb_ctx* ctx, hfb_env* env, hfb_robot* robot, size_t n_motions,
+                                    const double* d_q_from, const double* d_q_to, size_t n_self_pairs,
+                                    const uint32_t* self_pairs, size_t first_motion, size_t num_motions,
+                                    const hfb_collision_request* req, const hfb_validate_params* p,
+                                    const hfb_validate_out* d_out, void* stream) {
+  if (!ctx || !env || !robot ||
+      !validate_ok(n_motions, d_q_from, d_q_to, n_self_pairs, self_pairs, first_motion, num_motions, req, p, d_out))
+    return HFB_ERR_INVALID_ARGUMENT;
+  return env_call(ctx, env, Form::device, stream, 0, nullptr, nullptr,
+                  EnvValidateMotions{req, d_out, {0, n_self_pairs, self_pairs, 0, 0}, robot, n_motions, d_q_from,
+                                     d_q_to, first_motion, num_motions, *p});
 }
 
 // Each A object's nearest B object (hfb_env_distance_out in include/hppfcl_b200.h): the result of

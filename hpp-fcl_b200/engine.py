@@ -90,6 +90,8 @@ def load_library(path=None):
     L.hfb_robot_poses_device.argtypes = [vp, vp, sz, vp, vp, vp, vp]
     L.hfb_robot_sample_motions.argtypes = [vp, vp, sz, vp, vp, vp, vp]
     L.hfb_robot_sample_motions_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp]
+    L.hfb_env_validate_motions.argtypes = [vp, vp, vp, sz, vp, vp, sz, vp, sz, sz, vp, vp, vp]
+    L.hfb_env_validate_motions_device.argtypes = [vp, vp, vp, sz, vp, vp, sz, vp, sz, sz, vp, vp, vp, vp]
     L.hfb_comm_unique_id.argtypes = [vp]
     L.hfb_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
     L.hfb_comm_destroy.argtypes = [vp]
@@ -834,6 +836,55 @@ class Engine:
         out = P.RobotSamplesOut(d_tfs, d_handles, d_q, d_sweep)
         self._check(self.L.hfb_robot_sample_motions_device(self.h, robot, off.shape[0] - 1, _ptr(d_q_from), _ptr(d_q_to),
                                                            _ptr(off), C.byref(out), _ptr(stream)))
+
+    def env_validate_motions(self, env, robot, q_from, q_to, self_pairs, initial_depth, max_depth, max_samples, req=None,
+                             first_motion=0, num_motions=None):
+        """motion m from q_from[m] to q_to[m] ((n_motions, J) each) sampled by the robot, certified segment by segment
+        and the uncertified segments split until each motion is proven free, found colliding or at depth max_depth
+        (hfb_env_validate_motions) -> dict: status (0 valid, 1 collides, 2 unresolved, -1 outside the range), t_valid,
+        t_collide, the witness (kind, first, second, contacts) and the counts n_rounds, n_samples, n_env_candidates,
+        n_self_candidates, n_unsupported"""
+        req = req or P.CollisionRequestPOD()
+        J, _ = self.robot_dims(robot)
+        qf = np.ascontiguousarray(q_from, dtype=np.float64).reshape(-1)
+        qt = np.ascontiguousarray(q_to, dtype=np.float64).reshape(-1)
+        if qf.shape[0] % J or qt.shape[0] != qf.shape[0]:
+            raise ValueError("q_from, q_to: num_joints values per motion, as many motions in each")
+        tpl = _template(self_pairs)
+        n = qf.shape[0] // J
+        r = {"status": np.empty(n, dtype=np.int8), "t_valid": np.empty(n), "t_collide": np.empty(n),
+             "kind": np.empty(n, dtype=np.int8), "first": np.empty(n, dtype=np.uint32),
+             "second": np.empty(n, dtype=np.uint32), "contacts": np.empty(n, dtype=P.contact_dtype)}
+        rounds = np.zeros(1, dtype=np.uint32)
+        nc = np.zeros(4, dtype=np.uint64)
+        out = P.ValidateOut(*[r[k].ctypes.data for k in ("status", "t_valid", "t_collide", "kind", "first", "second",
+                                                         "contacts")], rounds.ctypes.data,
+                            *[nc[k:].ctypes.data for k in range(4)])
+        p = P.ValidateParams(int(initial_depth), int(max_depth), int(max_samples))
+        self._check(self.L.hfb_env_validate_motions(self.h, env, robot, n, _ptr(qf), _ptr(qt), tpl.shape[0], _ptr(tpl),
+                                                    first_motion, n - first_motion if num_motions is None else num_motions,
+                                                    C.byref(req), C.byref(p), C.byref(out)))
+        r["n_rounds"] = int(rounds[0])
+        for k, name in enumerate(("n_samples", "n_env_candidates", "n_self_candidates", "n_unsupported")):
+            r[name] = int(nc[k])
+        return r
+
+    def env_validate_motions_device(self, env, robot, n_motions, d_q_from, d_q_to, self_pairs, initial_depth, max_depth,
+                                    max_samples, d_status, d_t_valid, d_t_collide, d_kind=None, d_first=None,
+                                    d_second=None, d_contacts=None, d_counts=(None,) * 5, req=None, stream=0,
+                                    first_motion=0, num_motions=None):
+        """hfb_env_validate_motions_device: the end points and every output are device pointers, ordered on `stream`;
+        d_counts = (d_n_rounds (uint32), d_n_samples, d_n_env_candidates, d_n_self_candidates, d_n_unsupported
+        (uint64)); the template is a host array"""
+        req = req or P.CollisionRequestPOD()
+        tpl = _template(self_pairs)
+        out = P.ValidateOut(d_status, d_t_valid, d_t_collide, d_kind, d_first, d_second, d_contacts, *d_counts)
+        p = P.ValidateParams(int(initial_depth), int(max_depth), int(max_samples))
+        self._check(self.L.hfb_env_validate_motions_device(self.h, env, robot, int(n_motions), _ptr(d_q_from),
+                                                           _ptr(d_q_to), tpl.shape[0], _ptr(tpl), first_motion,
+                                                           n_motions - first_motion if num_motions is None
+                                                           else num_motions, C.byref(req), C.byref(p), C.byref(out),
+                                                           _ptr(stream)))
 
     @staticmethod
     def _objects(handles, tfs):

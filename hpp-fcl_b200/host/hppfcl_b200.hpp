@@ -984,11 +984,26 @@ class RobotModel {
     for (const CollisionGeometryPtr_t& g : geoms) C.handle(g.get());
     C.commit();
   }
+  friend class ResidentEnvironment;
   int device;
   Context& C;
   std::vector<CollisionGeometryPtr_t> geoms;
   hfb_robot* robot = nullptr;
   size_t nq_ = 0, L = 0;
+};
+
+/// What ResidentEnvironment::validate_motions returns: per motion status (0 valid, 1 collides, 2 unresolved, -1 outside
+/// the range), t_valid (the certified prefix is [0, t_valid]), t_collide (the earliest colliding sample found, -1 for
+/// none) and the witness there (kind, first, second: link indices, or an environment index for kind 0; contacts); the
+/// counts summed over the rounds.
+struct MotionValidation {
+  std::vector<int8_t> status;
+  std::vector<double> t_valid, t_collide;
+  std::vector<int8_t> kind;
+  std::vector<uint32_t> first, second;
+  std::vector<hfb_contact> contacts;
+  uint32_t n_rounds = 0;
+  uint64_t n_samples = 0, n_env_candidates = 0, n_self_candidates = 0, n_unsupported = 0;
 };
 
 /// config 5 in one call: the manager's candidate pairs through the batched narrow phase.  Returns, per candidate
@@ -1278,6 +1293,56 @@ class ResidentEnvironment {
                                     sweep.empty() ? &no_sweep : sweep.data(), links_per_config, self_pairs.size(),
                                     tpl.data(), n, offsets.data(), 0, n, &q, &o));
     return certified;
+  }
+
+  /// A planner's progressive motion validation: motion m runs from q_from[m] to q_to[m] (n_motions x nq each) of the
+  /// robot model, linear in q.  Each motion is cut into 2^initial_depth segments, certified as certify_motions
+  /// certifies them, and the uncertified segments are split again, down to 2^-max_depth of the motion, with at most
+  /// max_samples samples per round (hfb_env_validate_motions states the rounds and their guarantee).  Only motions
+  /// [first_motion, first_motion + num_motions) are validated (num_motions = SIZE_MAX: the rest).  q of the wrong size,
+  /// depths outside 0 <= initial_depth <= max_depth <= 30, max_samples < 2, a range past the end or a malformed
+  /// template throw std::invalid_argument.
+  MotionValidation validate_motions(RobotModel& robot, const std::vector<double>& q_from, const std::vector<double>& q_to,
+                                    const std::vector<std::pair<uint32_t, uint32_t>>& self_pairs, uint32_t initial_depth,
+                                    uint32_t max_depth, uint64_t max_samples,
+                                    const CollisionRequest& request = CollisionRequest(), size_t first_motion = 0,
+                                    size_t num_motions = SIZE_MAX) {
+    if (request.num_max_contacts == 0 && request.security_margin != -std::numeric_limits<FCL_REAL>::infinity())
+      throw std::invalid_argument("Invalid number of max contacts (current value is 0).");
+    if (initial_depth > max_depth || max_depth > 30 || max_samples < 2)
+      throw std::invalid_argument("need 0 <= initial_depth <= max_depth <= 30 and max_samples >= 2");
+    if (q_from.size() % robot.nq_ || q_to.size() != q_from.size())
+      throw std::invalid_argument("q_from, q_to: nq values per motion, as many motions in each");
+    const size_t n = q_from.size() / robot.nq_;
+    if (num_motions == SIZE_MAX) num_motions = first_motion <= n ? n - first_motion : 0;
+    if (first_motion > n || num_motions > n - first_motion) throw std::invalid_argument("motion range past the end");
+    hfb_collision_request q;
+    detail::fill(request, q);
+    std::vector<uint32_t> tpl;
+    for (const auto& p : self_pairs) {
+      tpl.push_back(p.first);
+      tpl.push_back(p.second);
+    }
+    robot.sync();
+    MotionValidation v;
+    v.status.resize(n);
+    v.t_valid.resize(n);
+    v.t_collide.resize(n);
+    v.kind.resize(n);
+    v.first.resize(n);
+    v.second.resize(n);
+    v.contacts.resize(n);
+    // no motions: the vectors may hand out null data(), which the C ABI refuses for the required outputs; one slot
+    // each stands in (nothing is written to it)
+    int8_t s0 = -1;
+    double tv0 = 0, tc0 = -1;
+    hfb_validate_out o{n ? v.status.data() : &s0, n ? v.t_valid.data() : &tv0, n ? v.t_collide.data() : &tc0,
+                       v.kind.data(), v.first.data(), v.second.data(), v.contacts.data(), &v.n_rounds, &v.n_samples,
+                       &v.n_env_candidates, &v.n_self_candidates, &v.n_unsupported};
+    const hfb_validate_params p{initial_depth, max_depth, max_samples};
+    C.check(hfb_env_validate_motions(C.raw(), env, robot.robot, n, q_from.data(), q_to.data(), self_pairs.size(),
+                                     tpl.data(), first_motion, num_motions, &q, &p, &o));
+    return v;
   }
 
  private:

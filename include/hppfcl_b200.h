@@ -730,8 +730,8 @@ int hfb_env_collide_motions_device(hfb_ctx* ctx, hfb_env* env, size_t n_a, const
  * so the guarantee weakens to "no pair penetrates deeper than |margin|" (BVH pairs are unsupported there).  For GJK
  * pairs the reference's lower bound is the converged distance, good to
  * gjk_tolerance only: a caller who wants strict slack adds 2 * gjk_tolerance to each sweep.
- * Refinement is the caller's: resample the segments with certified = 0 and call again (hpp-core's progressive
- * validation).  Handles, the env's validity and the request are checked as hfb_env_collide checks them.  A refused
+ * Refinement of the segments with certified = 0 is hfb_env_validate_motions' (hpp-core's progressive validation), or
+ * the caller's: resample them and call again.  Handles, the env's validity and the request are checked as hfb_env_collide checks them.  A refused
  * call (a null sweep or output, all three per-item outputs null, or a refusal of hfb_env_collide_motions) writes
  * nothing.
  *   hfb_env_certify_motions: HOST buffers, blocking.
@@ -848,6 +848,81 @@ int hfb_robot_sample_motions(hfb_ctx* ctx, hfb_robot* robot, size_t n_motions, c
 int hfb_robot_sample_motions_device(hfb_ctx* ctx, hfb_robot* robot, size_t n_motions, const double* d_q_from,
                                     const double* d_q_to, const uint32_t* motion_offsets,
                                     const hfb_robot_samples_out* d_out, void* cuda_stream);
+
+/* ---- a planner's progressive motion validation: each motion proven free, found colliding or left at its resolution --
+ * hfb_env_certify_motions over samples that hfb_robot_sample_motions would make, with the segments that fail
+ * certification split and checked again inside the call: hpp-core's continuous path validation
+ * (continuousValidation::Dichotomy / Progressive).  Motion m of n_motions runs from q_from[m*J ..] to q_to[m*J ..] (J the
+ * robot's joints), linear in q; the links are the robot's L links and the self-pair template is over link indices.
+ * Positions.  With D = max_depth, a sample sits at an integer position k in [0, 2^D], t = k * 2^-D; its joint values are
+ * q_from at k = 0, q_to at k = 2^D and q_from + t * (q_to - q_from) otherwise (hfb_robot_sample_motions' formula: t is an
+ * exact dyadic, so the samples of depth d are bit for bit those of 2^d + 1 samples).  A segment [a, b] of depth d has
+ * b - a = 2^(D-d); its sweep bounds are hfb_robot_sample_motions' bounds over q(a) -> q(b).
+ * Round 0 opens the 2^d0 segments of depth d0 = initial_depth of each motion of the range [first_motion, first_motion
+ * + num_motions).  A round:
+ *   1. Runs: each motion's open segments form runs, maximal chains of contiguous open segments; a run of s segments has
+ *      s + 1 samples.  Segments are admitted in (motion, position) order while the round's sample count stays <= the
+ *      cap: min(max_samples, 2^29, floor((2^32 - 1 - n_b) / L)), the last keeping samples * L + n_b below 2^32 as the
+ *      env calls' object counts are.
+ *   2. Certify: the runs go through one hfb_env_certify_motions as its motions, with the robot's poses at the samples
+ *      and the sweep bounds of the segments, the caller's request and template.
+ *   3. Collisions: c_m <- min(c_m, the first colliding sample of each of m's runs).
+ *   4. Segments: each open segment by the first rule that applies: certified -> closed; starts at or after c_m ->
+ *      dropped; not admitted, of depth D, or a link's sweep bound not finite (halving cannot make it finite) -> stuck;
+ *      otherwise split into two open halves.
+ *   5. Frontier: with f_m the start of m's earliest stuck segment, every open segment of m from f_m on is dropped.
+ * The call ends when no segment is open, after at most D - d0 + 1 rounds.  Per motion m of the range:
+ *   t_valid[m]:   the end of the prefix of certified segments (1 when every segment is certified).
+ *   t_collide[m]: c_m * 2^-D, -1 when no colliding sample was found.
+ *   status[m]:    1 (collides) when a colliding sample was found, else 0 (valid) when t_valid = 1, else 2 (unresolved).
+ *   kind, first, second, contacts: the witness at t_collide, what hfb_env_collide_motions returns for the one-sample
+ *                 motion q(t_collide) (first, second: link indices, or a B index for kind 0); the no-witness values
+ *                 without a colliding sample.  With all four null no witness is sought.
+ *   Motions outside the range: status -1, t_valid 0, t_collide -1 and the no-witness values.
+ *   n_rounds: the rounds that certified something; n_samples, n_env_candidates, n_self_candidates, n_unsupported: sums
+ *   over the rounds of their samples and of hfb_env_certify_motions' counts (64 bits wide).  Each count may be null.
+ * No output depends on scheduling.  For a colliding motion the first contact lies in (t_valid, t_collide].
+ * The guarantee: a valid motion is certified whole, and [0, t_valid] is free when t_valid > 0, under hfb_env_certify_motions' guarantee
+ * with its sweep bounds (including its weaker form under a negative security_margin and the gjk_tolerance caveat);
+ * security_margin == -inf behaves as there (no collide() runs, every segment with finite sweeps certified).
+ * Refusals, HFB_ERR_INVALID_ARGUMENT with nothing written: initial_depth > max_depth, max_depth > 30, max_samples < 2;
+ * a null context, env, robot, request, params, output struct, status, t_valid or t_collide; a null self_pairs with
+ * n_self_pairs > 0; null q_from / q_to with a non-empty range; a range past n_motions; then, under the context's lock,
+ * the request as hfb_env_collide checks it, the robot's refusals (hfb_robot_poses'), the env's, and the template's
+ * (hfb_env_collide_configs' with L the robot's link count).
+ *   hfb_env_validate_motions: HOST buffers, blocking.
+ *   hfb_env_validate_motions_device: q_from, q_to and every output in DEVICE memory (the template stays in host memory),
+ *     ordered on `cuda_stream`.  It blocks on `cuda_stream` once per round (the round's sample count sizes its
+ *     launches), where hfb_env_certify_motions_device blocks, and once more for the number of colliding motions;
+ *     growing a context or env buffer allocates device memory, which waits for the whole device. */
+typedef struct hfb_validate_params {
+  uint32_t initial_depth; /* d0: round 0 checks 2^d0 equal segments per motion */
+  uint32_t max_depth;     /* D, d0 <= D <= 30: no segment is shorter than 2^-D of its motion */
+  uint64_t max_samples;   /* per round, >= 2 */
+} hfb_validate_params;
+typedef struct hfb_validate_out {
+  int8_t* status;   /* n_motions: 0 valid, 1 collides, 2 unresolved; -1 outside the range */
+  double* t_valid;  /* n_motions: end of the certified prefix, in [0, 1] */
+  double* t_collide; /* n_motions: earliest colliding sample found, -1 if none */
+  int8_t* kind;     /* n_motions each: the witness at t_collide (may be null) */
+  uint32_t* first;
+  uint32_t* second;
+  hfb_contact* contacts;
+  uint32_t* n_rounds;
+  uint64_t* n_samples;
+  uint64_t* n_env_candidates;
+  uint64_t* n_self_candidates;
+  uint64_t* n_unsupported;
+} hfb_validate_out;
+int hfb_env_validate_motions(hfb_ctx* ctx, hfb_env* env, hfb_robot* robot, size_t n_motions, const double* q_from,
+                             const double* q_to, size_t n_self_pairs, const uint32_t* self_pairs, size_t first_motion,
+                             size_t num_motions, const hfb_collision_request* req, const hfb_validate_params* p,
+                             const hfb_validate_out* out);
+int hfb_env_validate_motions_device(hfb_ctx* ctx, hfb_env* env, hfb_robot* robot, size_t n_motions,
+                                    const double* d_q_from, const double* d_q_to, size_t n_self_pairs,
+                                    const uint32_t* self_pairs, size_t first_motion, size_t num_motions,
+                                    const hfb_collision_request* req, const hfb_validate_params* p,
+                                    const hfb_validate_out* d_out, void* cuda_stream);
 
 /* ---- object-table batches: the batched form of the CollisionObject overloads --------------------------
  * collide(const CollisionObject* o1, const CollisionObject* o2, ...) / distance(...) (include/hpp/fcl/collision.h:
